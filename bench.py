@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py — BASELINE.json's metric: MB/s ingested end to end, TF-IDF (benchmarks/tf-idf-dampr.py)
-on synthetic Zipf text, through the Dampr DSL on the B200 engine.
+on synthetic Zipf text, through the Dampr DSL on the H100 engine.
 
     python bench.py --gpus 1 --steps K --warmup W            # this engine
     python bench.py --impl reference --gpus 1 ...             # the reference's own CPU runner
@@ -22,6 +22,9 @@ the whole corpus (10 GB, V = 1e6, split evenly over the ranks: strong scaling).
                 6.25e8 16-byte records (32*N/t against the HBM peak), merge / reduce, config 2 end to end,
                 config 5 joins, the file-path e2e.
   cpu_baseline  the CPU arm on a bounded sample of the same corpus, all host cores.
+
+--dump-outputs DIR writes what the last timed end-to-end step computed (the sink rows of the TF-IDF job) as
+DIR/*.npy, so that two builds can be compared output for output: the inputs are seeded, identical from run to run.
 """
 import argparse
 import hashlib
@@ -38,6 +41,7 @@ import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True   # the tree may be read-only: the benchmark writes only to temporary directories
 
 import numpy as np
 
@@ -68,6 +72,8 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the kv / join / file-path extras (1 GPU)")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write the result of the last timed end-to-end step as DIR/<name>.npy (float64)")
     return ap.parse_args()
 
 
@@ -79,7 +85,7 @@ def dist_env():
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -155,7 +161,7 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "fallback"   # H100 SXM data sheet
 
 
 # ---- the CPU arms: the real reference (oracle/_ref, a separate process) or the oracle port ------------------------
@@ -328,7 +334,7 @@ def reference_arm(args):
         val = nbytes * len(times) / sum(times) / MB
         sample = "%d-byte line-aligned prefix of the synthetic corpus per step (oracle/gen.py, seed 1234, V=%d), %d worker processes on %d cores" % (
             nbytes, args.vocab, used, ncores)
-        how = ("the unmodified reference (pip install of /root/reference under oracle/_ref), benchmarks/tf-idf-dampr.py "
+        how = ("the unmodified reference (pip install under oracle/_ref), benchmarks/tf-idf-dampr.py "
                "statements, wall time of the whole python process" if kind == "reference"
                else "oracle/cpu_runner.py (port of the reference's runner; %s)" % (
                    ("the reference under oracle/_ref failed on this box: " + note) if note else "oracle/_ref is absent"))
@@ -441,6 +447,30 @@ def kv_extras(ctx_unused, args):
     guarded("config5", lambda: kv_bench.config5(ctx))
     guarded("config5_dsl", lambda: kv_bench.config5_dsl(ctx))
     return extra
+
+
+TFIDF_DUMP_ROWS = 2_000_000   # 3 float64 columns: at most 48 MB
+
+
+def dump_tfidf(out_dir, dump_dir, suffix=""):
+    """The sink rows of one TF-IDF run (term, document frequency, idf) in term order, as float64 arrays:
+    tfidf_term_hash (the first 48 bits of the term's blake2b digest, exact in float64), tfidf_doc_freq, tfidf_idf.
+    More than TFIDF_DUMP_ROWS rows are cut to a fixed, seeded sample of that many (still in term order)."""
+    rows = []
+    for line in read_sink_lines(out_dir):
+        term, df, idf = line.rsplit(b"\t", 2)
+        rows.append((term, int(df), float(idf)))
+    rows.sort()
+    if len(rows) > TFIDF_DUMP_ROWS:
+        keep = np.sort(np.random.default_rng(0).choice(len(rows), TFIDF_DUMP_ROWS, replace=False))
+        rows = [rows[i] for i in keep]
+    h = np.array([int.from_bytes(hashlib.blake2b(t, digest_size=6).digest(), "little") for t, _df, _idf in rows],
+                 dtype=np.float64)
+    os.makedirs(dump_dir, exist_ok=True)
+    np.save(os.path.join(dump_dir, "tfidf_term_hash%s.npy" % suffix), h)
+    np.save(os.path.join(dump_dir, "tfidf_doc_freq%s.npy" % suffix), np.array([r[1] for r in rows], dtype=np.float64))
+    np.save(os.path.join(dump_dir, "tfidf_idf%s.npy" % suffix), np.array([r[2] for r in rows], dtype=np.float64))
+    return len(rows)
 
 
 def file_e2e(Dampr, host_text, out_root, steps=2):
@@ -640,6 +670,10 @@ def main():
     elif os.environ.get("DAMPR_BENCH_PROFILE"):
         for i in range(5):
             step(True, 100 + i)
+
+    if args.dump_outputs:
+        n_dumped = dump_tfidf(d, args.dump_outputs, "_rank%d" % rank if world > 1 else "")
+        progress("dumped %d sink rows of the last timed step to %s" % (n_dumped, args.dump_outputs))
 
     # ---- full-size consistency: both timed variants produced the same result on every rank, the line
     # totals add up over the ranks -------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-"""dampr_b200 — B200-native map / shuffle / reduce engine behind the Dampr DSL.
+"""dampr_b200 — H100-native map / shuffle / reduce engine behind the Dampr DSL.
 
 Same public names as the reference package (dampr/__init__.py:14-33) so that
 ``from dampr_b200 import Dampr`` (or the ``dampr`` shim package) is a drop-in for

@@ -1,5 +1,6 @@
-"""Build libdampr_b200.so in-tree with nvcc for sm_100a (no JIT cache, the .so travels with the repo)."""
+"""Build libdampr_b200.so in-tree with nvcc for sm_90a (H100; no JIT cache, the .so travels with the repo)."""
 import os
+import shutil
 import subprocess
 import sys
 
@@ -7,8 +8,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdampr_b200.so")
 SOURCES = ["ctx.cu", "text.cu", "text2.cu", "kv.cu", "merge.cu", "ops.cu", "comm.cu"]
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [
     "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
 ]
 
@@ -19,7 +20,7 @@ def _newer(a, b):
 
 def build(force=False, verbose=False):
     """Compile every .cu into build/*.o and link the shared library. Returns the library path."""
-    nvcc = os.environ.get("NVCC", "nvcc")
+    nvcc = os.environ.get("NVCC") or shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
     objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
     deps = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "leaf.cuh"), os.path.join(HERE, "..", "include", "dampr_b200.h")]
@@ -36,7 +37,7 @@ def build(force=False, verbose=False):
             subprocess.check_call(cmd)
             relink = True
     if relink:
-        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-ldl"]
+        cmd = [nvcc, "-shared", "-o", LIB] + objs + ARCH + ["-ldl"]
         if verbose:
             print(" ".join(cmd), file=sys.stderr)
         subprocess.check_call(cmd)

@@ -1,4 +1,4 @@
-// common.cuh — shared declarations for libdampr_b200.so (sm_100a only).
+// common.cuh — shared declarations for libdampr_b200.so (sm_90a, H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,7 +16,7 @@ typedef uint32_t u32;
 typedef uint16_t u16;
 typedef uint8_t u8;
 
-#define DAMPR_NUM_SMS_DEFAULT 148
+#define DAMPR_NUM_SMS_DEFAULT 132
 
 struct TimedKernel {
     int id;

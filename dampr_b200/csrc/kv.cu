@@ -8,7 +8,7 @@
 //   ARReduce._reduce / Reduce     dampr/dampr.py:678-683, dampr/base.py:204-207  fold a group
 // (the k-way merge of sorted runs, MergeDataset.read dataset.py:571-579, lives in merge.cu)
 //
-// Design (B200), second generation:
+// Design, second generation:
 //   * ONE partition level of up to 12 key bits (4096 buckets) for up to ~1.1e8 records, then one
 //     leaf pass: two data passes instead of three.  A level is histogram -> scans -> scatter over
 //     per-CTA contiguous record ranges ("pieces"), so a bucket receives its records in input order

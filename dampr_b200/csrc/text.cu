@@ -6,7 +6,7 @@
 //                             benchmarks/tf-idf-dampr.py:12-14 (`set(RX.split(x.lower()))`)
 //   ReducedWriter.add_record  dampr/dataset.py:100-105  (dict combiner, binop = +1)
 //
-// Design (B200): persistent CTAs, 2 per SM. Each CTA owns 6 KB tiles of the text; a tile is
+// Design: persistent CTAs, 2 per SM. Each CTA owns 6 KB tiles of the text; a tile is
 // pulled into shared memory with one TMA 1-D bulk copy (cp.async.bulk + mbarrier), classified
 // 4 bytes at a time with SWAR arithmetic into bit masks (word chars, newlines), token starts are
 // ranked with a block scan, every token start is walked once to produce a 64-bit key code

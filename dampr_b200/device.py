@@ -203,7 +203,7 @@ class Ctx(object):
         rc = self.lib.dampr_ctx_create(int(device), C.byref(h))
         if rc:
             raise DeviceError(
-                "cannot create a device context on cuda:%d (status %d): the B200 engine needs a "
+                "cannot create a device context on cuda:%d (status %d): the engine needs a "
                 "CUDA device and has no CPU fallback" % (device, rc))
         self.h = h
         self.device = device

@@ -1,4 +1,4 @@
-"""The Dampr DSL on top of the B200 engine.
+"""The Dampr DSL on top of the device engine.
 
 Public surface = the reference's (dampr/dampr.py:19-977; SURVEY §8(b) "Python signatures to
 keep"): Dampr.memory/read_input/text/json/from_dataset/run, PMap.*, ARReduce.*, PReduce.*,
@@ -424,7 +424,7 @@ class PJoin(PBase):
 
 
 class Dampr(object):
-    """Entry point (dampr.py:831-957). `runner` defaults to the B200 runner and, unlike the
+    """Entry point (dampr.py:831-957). `runner` defaults to the device runner and, unlike the
     reference (SURVEY B7), is carried through every derived graph."""
 
     def __init__(self, graph=None, runner=None):

@@ -3,7 +3,7 @@
 Public names and call contracts follow the reference's operator layer (dampr/base.py:1-433:
 Mapper.map(*datasets), Streamable.stream(kvs), Reducer.reduce(*datasets), Combiner.combine,
 BlockMapper/BlockReducer start/add/finish) because users subclass them.  What differs is who
-executes them: the B200 runner (runner.py) recognises the structured descriptors (`Op`) that the
+executes them: the device runner (runner.py) recognises the structured descriptors (`Op`) that the
 DSL attaches to its own Map objects, lowers the closed set of idioms to CUDA pipelines and runs
 everything else as a host map that feeds the device shuffle.
 """

@@ -1,5 +1,5 @@
 /*
- * dampr_b200.h — C-ABI of libdampr_b200.so: the B200-native (sm_100a) replacement for the
+ * dampr_b200.h — C-ABI of libdampr_b200.so: the H100-native (sm_90a) replacement for the
  * hot path of Refefer/Dampr: map -> partition-by-key -> spill -> external merge sort ->
  * combiner/reduce.
  *

@@ -1,5 +1,5 @@
 """DSL parity on the GPU: the known-answer literals of the reference's own suite
-(reference tests/test_dampr.py, cited per test) re-stated against the B200 runner.  Every shuffle
+(reference tests/test_dampr.py, cited per test) re-stated against the device runner.  Every shuffle
 in here goes through libdampr_b200 (host map + device partition/sort, or a lowered pipeline)."""
 import heapq
 import itertools

@@ -1,6 +1,8 @@
 """GPU parity: text tokenise+combine kernels (csrc/text.cu) vs the oracle restatement.
 
 Bit-exact: counts, line counts, the '' token, key strings."""
+import os
+
 import numpy as np
 import pytest
 
@@ -128,19 +130,26 @@ def test_tile_boundaries(ctx):
 
 
 def test_flags(ctx, text_kernel):
-    if text_kernel == 1:
-        pytest.skip("limits below are those of the v2 kernel")
+    """The first-generation kernel (text.cu) keeps scan-wide flags in every mode: any '\\r' flags the scan and no
+    line is handed back; the [^\\w]+ lines that do not fit its window (6 KB + 4 KB halo) set TF_LONGLINE."""
     _, st = run_count(ctx, "café au lait\n".encode("utf-8"), dev.TOK_WS)
     assert st["flags"] & dev.TF_NONASCII
     _, st = run_count(ctx, b"a\r\nb\r\n", dev.TOK_WS)
     assert st["flags"] & dev.TF_CR          # str.split: scan-wide flag (token counts do not depend on it)
     _, st = run_count(ctx, b"a\r\nb\r\n", dev.TOK_NONWORD_LOWER_SET)
-    assert st["flags"] == 0 and st["fallback"] == 2   # [^\w]+ modes: the two lines go to the host, nothing else
+    if text_kernel == 1:
+        assert st["flags"] & dev.TF_CR and st["fallback"] == 0
+    else:
+        assert st["flags"] == 0 and st["fallback"] == 2   # [^\w]+ modes: the two lines go to the host, nothing else
     long_line = b"x " * 20000 + b"\n"
     _, st = run_count(ctx, b"a\n" * 4000 + long_line + b"b\n" * 4000, dev.TOK_NONWORD_LOWER_SET)
     assert st["flags"] & dev.TF_LONGLINE
     # more distinct tokens in one line than the de-duplication history holds
     many = b" ".join(b"w%d" % i for i in range(400)) + b"\n"
+    if text_kernel == 1:
+        check_df(ctx, b"a b\n" * 10 + many + b"c\n")
+        check_wc(ctx, b"a\n" * 4000 + long_line + b"b\n" * 4000)
+        return
     _, st = run_count(ctx, b"a b\n" * 10 + many + b"c\n", dev.TOK_NONWORD_LOWER_SET)
     assert st["flags"] & dev.TF_LONGLINE
     # both are fine for the first-generation kernel when they fit its 4 KB window
@@ -200,10 +209,21 @@ def test_per_line_fallback_lists_exactly_the_bad_lines(ctx, text_kernel):
     """[^\\w]+ tokenisers: a line holding a byte the device cannot tokenise like Python (non-ASCII, '\\r' in text
     mode) contributes nothing to the table / line count / '' count and is reported with its offset and length;
     everything else is counted as if those lines were not there."""
-    if text_kernel == 1:
-        pytest.skip("the first-generation kernel keeps scan-wide flags")
     lines = _bad_line_corpus()
     data = b"\n".join(lines) + b"\n"
+    if text_kernel == 1:
+        # the first-generation kernel keeps scan-wide flags: it hands no line back, the whole scan is the caller's
+        for mode in (dev.TOK_NONWORD_LOWER_SET, dev.TOK_NONWORD_LOWER):
+            tb = ctx.textbuf(len(data) + 64)
+            tb.upload_all(np.frombuffer(data, dtype=np.uint8))
+            tab = ctx.table(20)
+            tab.count(tb, 0, len(data), mode)
+            st = tab.stats()
+            assert st["flags"] & dev.TF_NONASCII and st["flags"] & dev.TF_CR and st["fallback"] == 0, st
+            assert len(tab.fallback_lines()) == 0
+            tb.free()
+            tab.free()
+        return
     for cr_is_data in (False, True):
         def is_bad(l):
             return any(b >= 0x80 for b in l) or (b"\r" in l and not cr_is_data)
@@ -250,8 +270,6 @@ def test_per_line_fallback_lists_exactly_the_bad_lines(ctx, text_kernel):
 
 
 def test_fallback_list_overflow_sets_the_scan_wide_flag(ctx, text_kernel):
-    if text_kernel == 1:
-        pytest.skip("v2 kernel only")
     data = "é\n".encode() * 70000      # more bad lines than the list holds (and than a warp region may isolate)
     _, st = run_count(ctx, data, dev.TOK_NONWORD_LOWER_SET, verify=False)
     assert st["flags"] & dev.TF_NONASCII
@@ -259,7 +277,8 @@ def test_fallback_list_overflow_sets_the_scan_wide_flag(ctx, text_kernel):
 
 def test_upload_file_through_cufile_matches_the_ring(ctx, tmp_path):
     """The opt-in cuFile ingest (dampr_set_option("file_cufile", 1), csrc/ctx.cu): the same bytes land in the text
-    buffer as through the page-locked ring; token counts agree. Skipped where libcufile cannot be opened."""
+    buffer as through the page-locked ring. Without the nvidia-fs driver the library refuses the path before it
+    loads libcufile, and the ring still serves the same buffer afterwards."""
     data = gen.text(31, 30000, V=5000)
     p = tmp_path / "c.txt"
     p.write_bytes(data)
@@ -276,6 +295,13 @@ def test_upload_file_through_cufile_matches_the_ring(ctx, tmp_path):
         try:
             tb2.upload_file(0, str(p), 0, len(data))
         except dev.DeviceError as e:
+            if not os.path.isdir("/proc/driver/nvidia-fs"):
+                assert "the nvidia-fs driver is not loaded" in str(e)
+                dev.set_option("file_cufile", 0)
+                tb2.upload_file(0, str(p), 0, len(data))
+                ctx.sync()
+                assert tb2.download(0, len(data)).tobytes() == data
+                return
             if "cuFile" in str(e):
                 pytest.skip("cuFile unavailable here: %s" % e)
             raise

@@ -25,7 +25,7 @@ def peak():
         with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"])
     except Exception:
-        return 6650.0
+        return 3350.0   # H100 SXM data sheet
 
 
 def agg(ctx):
@@ -183,7 +183,7 @@ def config2_e2e(ctx):
 
 def config4_scaled(ctx):
     """BASELINE config 4 at 1/5 scale (the full 50 GB run takes minutes with its input generation and checks:
-    tools/scale_check.py config4, profiles/r02_config4_three_jobs.json): group_by(k, v).reduce(sum) over 10 GB of
+    tools/scale_check.py config4): group_by(k, v).reduce(sum) over 10 GB of
     records (6.25e8, K = N/4) in host numpy columns with the device arena capped at 3.2 GB, so the job spills:
     12 batches -> sorted, pre-folded runs per key range in the host run buffer -> K5 merge per bucket. Three jobs:
     cold, second (run buffer kept), third (run buffer page-locked)."""
@@ -220,13 +220,13 @@ def config4_scaled(ctx):
     return {"what": "config 4 at 1/5 scale: group_by.reduce(sum) over 10 GB of host records through a 3.2 GB device arena "
                     "(spill path: sorted runs per batch -> host run buffer -> K5 merge per bucket)",
             "records": n, "arena_bytes": 3276 << 20, "runs": runs, "MB_per_s": runs[-1]["MB_per_s"],
-            "ok": all(r["ok"] for r in runs), "full_size": "profiles/r02_config4_three_jobs.json"}
+            "ok": all(r["ok"] for r in runs)}
 
 
 def config5(ctx):
-    """BASELINE config 5 at the C-ABI, device-resident: 20 GB (1.25e9) x 2 GB (1.25e8, unique keys) records,
+    """BASELINE config 5 at the C-ABI, device-resident: 10 GB (6.25e8) x 1 GB (6.25e7, unique keys) records,
     ~50 % of the left keys match: broadcast hash build + probe, and sort-merge join ranges."""
-    nl, nr = 1_250_000_000, 125_000_000
+    nl, nr = 625_000_000, 62_500_000
     L = ctx.synth_kv(1, nl, 2 * nr)
     R = ctx.synth_kv(2, nr, 4 * nr)
     ctx.sync()
@@ -257,7 +257,7 @@ def config5(ctx):
     R.free()
     Ru.free()
     probe_ms = kt.get("probe", 0.0)
-    return {"what": "config 5 (20 GB x 2 GB) at the C-ABI, device-resident", "left": nl, "right": nr, "build_unique": nbuild,
+    return {"what": "config 5 at 10 GB x 1 GB, at the C-ABI, device-resident", "left": nl, "right": nr, "build_unique": nbuild,
             "left_records_with_partner": hits, "both_joins_agree": bool(matched_records == hits),
             "probe": {"wall_s": round(wall_probe, 3), "kernels_ms": {a: round(b, 3) for a, b in kt.items()},
                       "algorithmic_GBps": round(16.0 * (nl + nbuild) / probe_ms / 1e6, 1) if probe_ms else None},
@@ -266,9 +266,9 @@ def config5(ctx):
             "join_ranges": {"wall_s": round(wall_join, 3), "kernels_ms": {a: round(b, 3) for a, b in kj.items()}, "left_groups": int(len(rows))}}
 
 
-def config5_dsl(ctx, nl=1_250_000_000, nr=125_000_000):
-    """BASELINE config 5 through the DSL: L.group_by(k, v).join(R.group_by(k, v)) with HOST numpy columns (20 GB x
-    2 GB at the default sizes), the right side a dimension table with unique keys, half of the left keys matching:
+def config5_dsl(ctx, nl=625_000_000, nr=62_500_000):
+    """BASELINE config 5 through the DSL: L.group_by(k, v).join(R.group_by(k, v)) with HOST numpy columns (10 GB x
+    1 GB at the default sizes, what an 80 GB H100 joins without spilling), the right side a dimension table with unique keys, half of the left keys matching:
     reduce(lambda l, r: itertools.product(l, r), many=True) — the broadcast hash build + probe — and
     reduce(lambda l, r: (sum(l), sum(r))) — per-side device folds + probe of the group keys. Wall times include
     the H2D upload of both sides and the D2H of the result columns; the results are checked against each other and
