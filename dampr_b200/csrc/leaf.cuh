@@ -11,15 +11,11 @@ constexpr int L_BINS = 8192;   // counting-sort bins
 constexpr int L_IPT = L_CAP / L_THREADS;  // 8
 constexpr int L_HEAVY = 32;    // bins above this population are sorted by a warp when they hold one key
 
-constexpr int CL = 8;           // CTAs per leaf cluster
-constexpr int CF = 256;         // fine bins of the in-cluster exchange
-
 // ---- leaves ------------------------------------------------------------------------------------------
 struct LeafChunk {
     u64 start;      // first record
-    u32 n;          // records (<= L_CAP for the single-CTA leaf, <= C_NMAX for the cluster leaf)
-    int bin_shift;  // single CTA: bin = ((xf(key) - base) >> bin_shift) - bin_base
-                    // cluster   : fine bin = ((xf(key) - base) >> bin_shift) - bin_base, in [0, 256)
+    u32 n;          // records, <= L_CAP
+    int bin_shift;  // bin = ((xf(key) - base) >> bin_shift) - bin_base
     u64 bin_base;
     u32 entry;      // first entry of the chunk in the (start, groups) table of the reduce path
     u32 pad;
@@ -31,15 +27,13 @@ struct LeafSmem {
     u16 cnt[L_BINS];  // counts, then bin starts (hash path: slot -> record index + 1)
     u16 ord[L_CAP];   // bin order -> record index (hash path: representative flags)
     u16 fin[L_CAP];   // final order -> record index
-    u16 aux[L_CAP];   // cluster leaf: index of the record inside its chunk (the stable tie-break)
-    // cluster exchange
-    u32 fh[CF];
-    u32 gpos[CF + 1];
-    u16 dpos[CF];
-    u32 firstg[CL], endg[CL];
+    u32 heavy_bm[(L_THREADS / 32) * (L_CAP / 32)];  // leaf_sort_heavy_bins: per warp, a presence bitmap of record indices
+    u32 heavy_flag[L_BINS / 32];                    // leaf_sort_heavy_bins: a bit per heavy bin that holds one key
+    // Unused bytes that keep `wsum` at its offset. Moving it makes ptxas schedule leaf_sort_kernel and
+    // merge_tile_kernel differently: on an H100 80GB HBM3 at 700 W, the leaves of a 1e8-record sort took 8 %
+    // less time and an 8-run merge of 1e8 records 0.4 % more. That trade is for a change of its own.
+    u32 unused[401];
     u32 wsum[32];
-    u32 total_groups;
-    u32 ovf;
 };
 
 __device__ __forceinline__ u64 apply_op(int op, u64 acc, u64 v) {
@@ -163,12 +157,10 @@ __device__ __forceinline__ bool leaf_bin_records(LeafSmem &s, u32 n, int bin_shi
 // Heavy bins (many records of ONE key: duplicate-heavy inputs) would cost every member a walk over the whole
 // bin. A warp checks that the bin holds a single key and, if so, sorts the bin's record indices through a
 // presence bitmap (O(members + 128)); the bin is flagged and its members take their rank by binary search.
-// Scratch: the cluster-exchange fields, unused outside the cluster leaf (s.aux = 16 bitmaps, s.fh = flags).
 __device__ __forceinline__ void leaf_sort_heavy_bins(LeafSmem &s, u32 n) {
     const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    u32 *flags = s.fh;                                                    // L_BINS bits
-    u32 *bm = reinterpret_cast<u32 *>(s.aux) + warp * (L_CAP / 32);       // L_CAP bits per warp
-    static_assert(sizeof(s.fh) * 8 >= L_BINS && sizeof(s.aux) >= (L_THREADS / 32) * (L_CAP / 8), "scratch too small");
+    u32 *flags = s.heavy_flag;
+    u32 *bm = s.heavy_bm + warp * (L_CAP / 32);
     if (tid < L_BINS / 32) flags[tid] = 0;
     __syncthreads();
     constexpr u32 BPW = L_BINS / (L_THREADS / 32);  // bins per warp
@@ -222,16 +214,14 @@ __device__ __forceinline__ void leaf_sort_heavy_bins(LeafSmem &s, u32 n) {
     __syncthreads();
 }
 
-// second half: the final position of record i — its bin's start plus its rank inside the bin by (key, tie-break),
-// the tie-break being the record's smem index (input position) or, in the cluster leaf, its index inside the
-// chunk (s.aux)
-template <bool HAS_AUX>
+// second half: the final position of record i — its bin's start plus its rank inside the bin by (key, smem index),
+// the smem index being the record's input position
 __device__ __forceinline__ u32 leaf_final_pos(const LeafSmem &s, u32 n, u32 i, u32 slotinfo, bool heavy = false) {
     const u32 bin = slotinfo >> 16;
     const u32 st = s.cnt[bin];
     const u32 en = (bin + 1 < L_BINS) ? s.cnt[bin + 1] : n;
     u32 r = 0;
-    if (!HAS_AUX && heavy && en - st > (u32)L_HEAVY && ((s.fh[bin >> 5] >> (bin & 31)) & 1u)) {
+    if (heavy && en - st > (u32)L_HEAVY && ((s.heavy_flag[bin >> 5] >> (bin & 31)) & 1u)) {
         // single-key bin whose indices a warp sorted (leaf_sort_heavy_bins): rank = lower bound of my index
         u32 lo = st, hi = en;
         while (lo < hi) {
@@ -243,29 +233,25 @@ __device__ __forceinline__ u32 leaf_final_pos(const LeafSmem &s, u32 n, u32 i, u
     }
     if (en - st > 1) {
         const u64 ki = s.sk[i];
-        const u32 ti = HAS_AUX ? s.aux[i] : i;
         for (u32 j = st; j < en; ++j) {
             const u32 o = s.ord[j];
             const u64 ko = s.sk[o];
-            const u32 to = HAS_AUX ? s.aux[o] : o;
-            r += (ko < ki || (ko == ki && to < ti)) ? 1u : 0u;
+            r += (ko < ki || (ko == ki && o < i)) ? 1u : 0u;
         }
     }
     return st + r;
 }
 
 // Sort the n records held in s.sk / s.val. Result: s.fin[position] = record index.
-template <bool HAS_AUX>
 __device__ __forceinline__ void leaf_sort_core(LeafSmem &s, u32 n, int bin_shift, u64 bin_base) {
     const u32 tid = threadIdx.x;
     u32 slot[L_IPT];
-    bool heavy = leaf_bin_records(s, n, bin_shift, bin_base, slot);
-    if (HAS_AUX) heavy = false;
+    const bool heavy = leaf_bin_records(s, n, bin_shift, bin_base, slot);
     if (heavy) leaf_sort_heavy_bins(s, n);
 #pragma unroll
     for (int k = 0; k < L_IPT; ++k) {
         const u32 i = tid + k * L_THREADS;
-        if (i < n) s.fin[leaf_final_pos<HAS_AUX>(s, n, i, slot[k], heavy)] = (u16)i;
+        if (i < n) s.fin[leaf_final_pos(s, n, i, slot[k], heavy)] = (u16)i;
     }
     __syncthreads();
 }

@@ -154,7 +154,7 @@ merge_tile_kernel(const RunDesc *__restrict__ runs, u32 k, const u64 *__restrict
             const u64 span = bkeys[p + 1] - klo;
             int shift = 0;
             while (shift < 64 && (span >> shift) >= (u64)L_BINS) ++shift;
-            leaf_sort_core<false>(s, n, shift, 0);
+            leaf_sort_core(s, n, shift, 0);
         } else {
             for (u32 i = tid; i < n; i += L_THREADS) s.fin[i] = (u16)i;
             __syncthreads();

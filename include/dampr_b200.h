@@ -42,12 +42,14 @@ typedef struct dampr_kv dampr_kv;           /* device array of 16-byte (u64 key,
 /* ---- library ------------------------------------------------------------------------- */
 int32_t dampr_abi_version(void);
 int32_t dampr_device_count(int32_t *out_n);
-/* process-wide tuning switches: "kv_scatter" (2 = atomic-rank scatter, up to 12 digit bits per level,
- * default; 1 = first-generation ballot scatter, 10 bits), "kv_cluster" (1 = thread-block-cluster leaf over
- * distributed shared memory, default), "kv_tile" (4096 | 8192 records per scatter tile), "kv_max_bits";
- * "scatter_tma" (first-generation scatter only: 1 = TMA bulk stores, 0 = coalesced 16-byte stores); "text_ctas" (3 = single-window 3 CTAs/SM variant of the v2
- * tokenise kernel, default; 2 = double-buffered 2 CTAs/SM); "text_kernel" (2 = warp-autonomous tokenise kernel, default;
- * 1 = first-generation kernel, also the fallback for lines longer than 2 KB) */
+/* process-wide tuning switches; any other name, or a value out of range, returns DAMPR_ERR_ARG:
+ *   "text_ctas"      2..4, default 4: resident CTAs per SM of the warp-autonomous tokenise kernel
+ *   "text_kernel"    1 | 2, default 2: 2 = warp-autonomous tokenise kernel; 1 = first-generation kernel, also
+ *                    the fallback for lines longer than 2 KB
+ *   "host_threads"   1..256, default 16: upper bound on the copy threads of a staged host transfer
+ *   "file_cufile"    0 | 1, default 0: 1 = file ingest through cuFile (GPUDirect Storage) instead of the
+ *                    page-locked ring
+ *   "cufile_threads" 1..64, default 8: reader threads of the cuFile ingest */
 int32_t dampr_set_option(const char *name, int64_t value);
 
 /* ---- context: replaces the process pool of StageRunner.run (stagerunner.py:15-43) ---- */

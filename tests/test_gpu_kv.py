@@ -280,37 +280,26 @@ def test_synth_kv_matches_numpy(ctx):
     assert np.array_equal(k2, ek) and np.array_equal(v2.view(np.int64), ev)
 
 
-# ---- second-generation sort path: 12-bit atomic-rank scatter + cluster/DSMEM leaf + K5 merge ----------------
+# ---- partition level + CTA leaf at chosen sizes, recursion on oversized segments ---------------------------
 @pytest.mark.parametrize("n", [4097, 9000, 27000, 27600, 60000, 1_000_000])
-def test_cluster_leaf_sizes(ctx, n):
-    """sizes around the single-CTA / cluster / one-level boundaries, unique-ish and duplicated keys, with the
-    default leaves and with the cluster (DSMEM) leaf"""
-    for cluster in (0, 1):
-        dev.set_option("kv_cluster", cluster)
-        try:
-            for nk in (max(1, n // 3), 10 * n):
-                keys, vals = gen.kv(77, n, nk)
-                check_sort(ctx, keys, vals, dev.KEY_MIX)
-                check_sort(ctx, keys, vals, dev.KEY_RAW)
-        finally:
-            dev.set_option("kv_cluster", 0)
+def test_sort_sizes_around_leaf_and_level_boundaries(ctx, n):
+    """4097 is the smallest input that needs a partition level (one leaf holds 4096 records); the larger sizes
+    fill the leaf chunks unevenly, up to 1M records in one level; unique-ish and duplicated keys"""
+    for nk in (max(1, n // 3), 10 * n):
+        keys, vals = gen.kv(77, n, nk)
+        check_sort(ctx, keys, vals, dev.KEY_MIX)
+        check_sort(ctx, keys, vals, dev.KEY_RAW)
 
 
-def test_cluster_leaf_overflow_falls_back(ctx):
-    """a chunk the cluster cannot balance (one key holds most of a 20K-record bucket) is re-sorted exactly"""
+def test_one_key_holding_most_of_a_bucket(ctx):
+    """one key holds 70 % of a 20K-record input: its segment outgrows a leaf and is sorted by recursion, where
+    the all-equal remainder is copied or folded as one group; the order stays stable and the folds see every
+    record"""
     rng = np.random.default_rng(5)
     n = 20000
     keys = rng.integers(0, 1 << 62, size=n).astype(np.uint64)
     keys[rng.random(n) < 0.7] = np.uint64(123456789)
     vals = np.arange(n, dtype=np.int64)
-    dev.set_option("kv_cluster", 1)
-    try:
-        _overflow_checks(ctx, keys, vals)
-    finally:
-        dev.set_option("kv_cluster", 0)
-
-
-def _overflow_checks(ctx, keys, vals):
     check_sort(ctx, keys, vals, dev.KEY_MIX)
     check_sort(ctx, keys, vals, dev.KEY_RAW)
     kv = ctx.kv_from_columns(keys, vals)
@@ -323,26 +312,16 @@ def _overflow_checks(ctx, keys, vals):
     assert dict(zip(k2.tolist(), v2.view(np.int64).tolist())) == refsem.group_fold(keys, vals, lambda a, b: a)
 
 
-@pytest.mark.parametrize("opts", [{"kv_hist": 1}, {"kv_scatter": 3}, {"kv_scatter": 2}, {"kv_cluster": 1},
-                                  {"kv_scatter": 2, "kv_cluster": 1, "kv_hints": 0}, {"kv_scatter": 2, "kv_max_bits": 11},
-                                  {"kv_scatter": 3, "kv_cluster": 1}])
-def test_sort_variants_agree(ctx, opts):
-    """every selectable kernel variant gives the same stable order (and leaves the defaults restored)"""
-    defaults = {"kv_scatter": 1, "kv_hist": 2, "kv_cluster": 0, "kv_hints": 1, "kv_max_bits": 12}
-    try:
-        for k, v in opts.items():
-            dev.set_option(k, v)
-        keys, vals = gen.kv(13, 2_500_000, 700_000)
-        check_sort(ctx, keys, vals, dev.KEY_MIX)
-        keys = (np.random.default_rng(3).zipf(1.2, size=600_000) % 5000).astype(np.uint64)
-        check_sort(ctx, keys, np.arange(len(keys), dtype=np.int64), dev.KEY_RAW)
-        kv = ctx.kv_from_columns(keys, np.ones(len(keys), dtype=np.int64))
-        out = kv.sort_reduce(dev.OP_SUM_I64, dev.KEY_MIX)
-        k2, v2 = out.columns()
-        assert dict(zip(k2.tolist(), v2.tolist())) == refsem.group_count(keys)
-    finally:
-        for k, v in defaults.items():
-            dev.set_option(k, v)
+def test_sort_mixed_and_zipf_keys_and_counts(ctx):
+    """a 2.5M-record KEY_MIX sort, a Zipf-skewed KEY_RAW sort and the sort_reduce counts of the Zipf keys"""
+    keys, vals = gen.kv(13, 2_500_000, 700_000)
+    check_sort(ctx, keys, vals, dev.KEY_MIX)
+    keys = (np.random.default_rng(3).zipf(1.2, size=600_000) % 5000).astype(np.uint64)
+    check_sort(ctx, keys, np.arange(len(keys), dtype=np.int64), dev.KEY_RAW)
+    kv = ctx.kv_from_columns(keys, np.ones(len(keys), dtype=np.int64))
+    out = kv.sort_reduce(dev.OP_SUM_I64, dev.KEY_MIX)
+    k2, v2 = out.columns()
+    assert dict(zip(k2.tolist(), v2.tolist())) == refsem.group_count(keys)
 
 
 def test_low_cardinality_keys_hot_runs(ctx):

@@ -136,6 +136,19 @@ def test_abi_exports_every_declared_symbol():
     dev.load_library()
 
 
+def test_set_option_accepts_only_the_live_switches():
+    """The partition/sort kernel variants and their switches are gone: their names are unknown options. The
+    switches that remain accept their defaults (setting them leaves the process as it was). Each removed name
+    is tried with the value that was its default."""
+    for name, old_default in (("kv_scatter", 1), ("kv_hist", 2), ("kv_cluster", 0), ("kv_hints", 1),
+                              ("kv_max_bits", 12), ("kv_leaf_target", 2600), ("scatter_tma", 1)):
+        with pytest.raises(dev.DeviceError):
+            dev.set_option(name, old_default)
+    for name, default in (("text_ctas", 4), ("text_kernel", 2), ("host_threads", 16), ("file_cufile", 0),
+                          ("cufile_threads", 8)):
+        dev.set_option(name, default)
+
+
 def test_no_gpu_fails_loudly():
     if dev.device_count() > 0:
         pytest.skip("GPU present")

@@ -17,9 +17,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from dampr_b200 import device as dev
 
 
-DEFAULTS = {"kv_scatter": 1, "kv_hist": 2, "kv_cluster": 0, "kv_hints": 1, "kv_max_bits": 12}
-
-
 def peak():
     try:
         with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")) as f:
@@ -315,22 +312,9 @@ def config5_dsl(ctx, nl=625_000_000, nr=62_500_000):
 
 def main():
     sizes = [float(x) for x in sys.argv[1:] if not x.startswith("-")] or [100.0]
-    variants = "--variants" in sys.argv
     ctx = dev.Ctx(0)
     for m in sizes:
         n = int(m * 1e6)
-        if variants:
-            for opts, label in (({"kv_scatter": 1, "kv_hist": 1}, "round 1: ballot scatter 2 x 8b + first histogram + CTA leaf"),
-                                ({"kv_scatter": 2, "kv_cluster": 1}, "table scatter 12b + cluster (DSMEM) leaf"),
-                                ({"kv_scatter": 3}, "staged scatter, atomic + SWAR ranking, 2 x 8b + CTA leaf"),
-                                ({}, "default: ballot scatter 2 x 8b + unrolled histogram + CTA leaf (direct emit)")):
-                for a, b in DEFAULTS.items():
-                    dev.set_option(a, b)
-                for a, b in opts.items():
-                    dev.set_option(a, b)
-                print(json.dumps(sort_case(ctx, n, n, label=label)), flush=True)
-            for a, b in DEFAULTS.items():
-                dev.set_option(a, b)
         print(json.dumps(sort_case(ctx, n, n, label="K=N")), flush=True)
         print(json.dumps(sort_case(ctx, n, 10_000_000, label="K=1e7")), flush=True)
         print(json.dumps(reduce_case(ctx, n, 10_000_000, label="K=1e7")), flush=True)

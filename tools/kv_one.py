@@ -1,6 +1,6 @@
 """One pass of each kv hot kernel on device-resident synthetic records, for ncu captures:
-    ncu --set full --import-source on --clock-control none -k regex:"part_scatter2|cluster_leaf|merge_tile|part_hist2" \
-        -c 8 -o gpurun_out/r02_kv python tools/kv_one.py 40"""
+    ncu --set full --import-source on --clock-control none \
+        -k regex:"part_hist2|part_scatter|leaf_sort|merge_tile" -c 8 -o kv_one python tools/kv_one.py 40"""
 import os
 import sys
 

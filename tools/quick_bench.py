@@ -74,28 +74,26 @@ def main():
     if kv_mrec > 0:
         n = int(kv_mrec * 1e6)
         for nk, label in ((10_000_000, "K=1e7"), (n, "K=N")):
-            for tma in (1, 0):
-                dev.set_option("scatter_tma", tma)
-                kv = ctx.kv(n)
-                ctx.check(ctx.lib.dampr_synth_kv(ctx.h, kv.h, 42, n, nk))
-                ctx.sync()
-                ctx.timings_reset()
-                t0 = time.time()
-                kv.sort(dev.KEY_MIX)
-                ctx.sync()
-                wall = time.time() - t0
-                summarize(ctx, "kv_sort[%s tma=%d] n=%d wall=%.1fms" % (label, tma, n, wall * 1e3), 32 * n)
-                ctx.check(ctx.lib.dampr_synth_kv(ctx.h, kv.h, 42, n, nk))
-                ctx.sync()
-                ctx.timings_reset()
-                t0 = time.time()
-                out = kv.sort_reduce(dev.OP_SUM_I64, dev.KEY_MIX)
-                ctx.sync()
-                wall = time.time() - t0
-                summarize(ctx, "kv_sort_reduce[%s tma=%d] n=%d groups=%d wall=%.1fms" % (label, tma, n, len(out), wall * 1e3),
-                          16 * n + 16 * len(out))
-                out.free()
-                kv.free()
+            kv = ctx.kv(n)
+            ctx.check(ctx.lib.dampr_synth_kv(ctx.h, kv.h, 42, n, nk))
+            ctx.sync()
+            ctx.timings_reset()
+            t0 = time.time()
+            kv.sort(dev.KEY_MIX)
+            ctx.sync()
+            wall = time.time() - t0
+            summarize(ctx, "kv_sort[%s] n=%d wall=%.1fms" % (label, n, wall * 1e3), 32 * n)
+            ctx.check(ctx.lib.dampr_synth_kv(ctx.h, kv.h, 42, n, nk))
+            ctx.sync()
+            ctx.timings_reset()
+            t0 = time.time()
+            out = kv.sort_reduce(dev.OP_SUM_I64, dev.KEY_MIX)
+            ctx.sync()
+            wall = time.time() - t0
+            summarize(ctx, "kv_sort_reduce[%s] n=%d groups=%d wall=%.1fms" % (label, n, len(out), wall * 1e3),
+                      16 * n + 16 * len(out))
+            out.free()
+            kv.free()
     ctx.close()
 
 
