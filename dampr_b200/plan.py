@@ -862,7 +862,27 @@ _FOLD_OPS = {lowering.ADD: dev.OP_SUM_I64, lowering.MIN: dev.OP_MIN_I64, lowerin
 
 
 def _key_xform_for(col):
-    return dev.KEY_I64 if col.dtype == np.int64 else dev.KEY_RAW
+    if col.dtype == np.int64:
+        return dev.KEY_I64
+    return dev.KEY_F64 if col.dtype == np.float64 else dev.KEY_RAW
+
+
+def _float_keys(col):
+    """A float64 key column as Python compares keys: (col + 0.0, the key its 0.0 group reports), or None when the
+    column holds a NaN (NaN != NaN: no sort or grouping of bit patterns gives Python's answer). -0.0 == 0.0 are
+    one key, and a group reports the key of its first record in input order, as the reference does."""
+    if np.isnan(col).any():
+        return None
+    zero = np.flatnonzero(col == 0)
+    return col + 0.0, (col[zero[0]] if len(zero) else np.float64(0.0))
+
+
+def _report_zero(keys, rep):
+    """group keys of a column normalised by _float_keys, with the 0.0 group relabelled to the key it reports"""
+    if np.signbit(rep):
+        keys = keys.copy()
+        keys[keys == 0] = rep
+    return keys
 
 
 def _lower_kv_map(runner, stage, inputs):
@@ -885,6 +905,20 @@ def _lower_kv_map(runner, stage, inputs):
         if stage.combiner is not None:
             return None
         col, other = cols[kp[1]], cols[1 - kp[1]]
+        if col.dtype == np.float64:
+            # sorted on the normalised key with the record positions as values: -0.0 and 0.0 tie (input order
+            # kept), and the rows are gathered from the input, so a -0.0 field stays -0.0
+            fk = _float_keys(-col if kp[2] < 0 else col)
+            if fk is None:
+                return None
+            kn, rep = fk
+            _k, perm, how = _device_group(runner, kn.view(np.uint64), np.arange(len(col), dtype=np.uint64), None,
+                                          dev.KEY_F64)
+            perm = perm.view(np.int64)
+            rk, ro = col[perm], other[perm]
+            f = Frame(_report_zero(kn[perm], rep), [rk, ro] if kp[1] == 0 else [ro, rk], scalar=False, combined=False)
+            runner.stats.add(stage, "device kv partition+sort of whole records" + how, "records=%d" % len(col))
+            return f
         if kp[2] < 0:
             if col.dtype != np.int64 or (len(col) and int(col.min()) == -(1 << 63)):
                 return None
@@ -900,6 +934,12 @@ def _lower_kv_map(runner, stage, inputs):
     if kp[2] != 1:
         return None
     keys = cols[kp[1]]
+    rep = None
+    if keys.dtype == np.float64:
+        fk = _float_keys(keys)
+        if fk is None:
+            return None
+        keys, rep = fk
     count_only = False
     if vp[0] == "field" and vp[2] == 1 and vp[1] in (0, 1):
         vals = cols[vp[1]]
@@ -930,13 +970,17 @@ def _lower_kv_map(runner, stage, inputs):
             overflow = chk.result() if chk is not None else False
         if overflow:
             raise NotLowerable("64-bit sum could overflow (SURVEY B12)")
-        f = Frame(rk.view(keys.dtype), [rv.view(np.int64)], scalar=True, combined=True)
+        rk = rk.view(keys.dtype)
+        f = Frame(rk if rep is None else _report_zero(rk, rep), [rv.view(np.int64)], scalar=True, combined=True)
         runner.stats.add(stage, "device kv partition+sort+segmented-reduce" + how, "records=%d groups=%d" % (n, len(rk)))
         return f
     if stage.combiner is None:
         # group_by: the partition + sort is deferred until somebody reads the grouped records; when the
         # only consumer is a lowered reduce (sum(it), len, min, max) the sort and the fold run as ONE
-        # device pass (or one spill pipeline) over the original columns
+        # device pass (or one spill pipeline) over the original columns. Its consumers (fused reduces, unique,
+        # joins) report the normalised keys, so a 0.0 group whose first key is -0.0 is left to the host
+        if rep is not None and np.signbit(rep):
+            return None
         f = LazyKVFrame(runner, keys, vals, _key_xform_for(keys))
         f.meta["sorted_kv"] = True
         runner.stats.add(stage, "device kv partition+sort (deferred until read; fused into a lowered reduce)",
@@ -1176,8 +1220,11 @@ def _lower_frame_map(runner, stage, frame):
             return None
         sign = kp[2]
         if col.dtype.kind == "f":
-            kcol = (col * sign) if sign < 0 else col
-            codes, xf = kcol.view(np.uint64), dev.KEY_F64
+            fk = _float_keys(-col if sign < 0 else col)
+            if fk is None:
+                return None
+            kcol = _report_zero(*fk)
+            codes, xf = fk[0].view(np.uint64), dev.KEY_F64
         else:
             kcol = (-col.astype(np.int64)) if sign < 0 else col.astype(np.int64)
             codes, xf = kcol.view(np.uint64), dev.KEY_I64
@@ -1225,6 +1272,9 @@ def _fold_column(runner, kcodes, xf, vals, kind):
         raise NotLowerable("fold %s" % kind)
     if kind == lowering.ADD and vals.dtype == np.int64 and len(vals) and _may_overflow(vals):
         raise NotLowerable("64-bit sum could overflow (SURVEY B12)")
+    if kind in (lowering.MIN, lowering.MAX) and vals.dtype == np.float64 and \
+            (np.isnan(vals).any() or (np.signbit(vals) & (vals == 0)).any()):
+        raise NotLowerable("NaN or -0.0 under min/max")   # Python's answer depends on the order of the arguments
     rk, rv, how = _device_group(runner, kcodes, vals.view(np.uint64), opmap[kind], xf)
     return rk, rv.view(vals.dtype), how
 
