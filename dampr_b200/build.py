@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdampr_b200.so")
-SOURCES = ["ctx.cu", "text.cu", "text2.cu", "kv.cu", "merge.cu", "ops.cu", "comm.cu"]
+SOURCES = ["ctx.cu", "text.cu", "text2.cu", "fields.cu", "kv.cu", "merge.cu", "ops.cu", "comm.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [
     "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",

@@ -1,0 +1,395 @@
+// fields.cu — delimited-field scan + combine: `line.split(sep)[i]` keys folded with a count, an int sum, a minimum
+// or a maximum of `int(line.split(sep)[j])`.
+//
+// Replaces, for the lowered field idioms, the reference's per-record Python in the map stage:
+//   TextLineDataset.read      dampr/dataset.py:458-476  (line ownership, '\n' stripping)
+//   Map.stream(user lambdas)  dampr/base.py:30-33 with `l.split(S)[i]` keys and `1` / `int(l.split(S)[j])` values
+//   ReducedWriter.add_record  dampr/dataset.py:100-105  (dict combiner with binop +, min or max)
+//
+// Design: persistent CTAs. A CTA copies a 16 KB tile of the text (plus a 4 KB halo) into shared memory, finds the
+// lines whose first byte lies in the tile (newline masks, one block scan that compacts their starts), then gives
+// one line to each thread. A thread walks its line 4 bytes per step with SWAR masks for separator, newline and the
+// bytes the device does not take; it resolves the key and value fields (negative indices count the separators
+// first), builds the key code, parses the value and does ONE insert into the global (L2-resident) combiner table.
+// There is one table operation per line, not one per token, so no shared-memory combiner sits in front of it.
+// HBM traffic = the text, read once.
+//
+// Key codes: a str key of 1..9 bytes packs 7 bits per byte (the str.split code of the tokeniser, so the table's
+// word decoding applies unchanged); '' and longer keys take the seeded hash with bit 63 set and a representative
+// (offset << 20 | length) that every later occurrence is byte-compared with (DAMPR_TF_COLLISION on a mismatch).
+// '' would pack to 0, the table's empty-slot marker: it goes through the hashed path with a length-0
+// representative. An int key v (|v| < 10^18) is v ^ 2^63: never 0, ordered like a signed int.
+//
+// Accumulators: SUM adds two's-complement values. MIN and MAX keep an order-preserving code whose identity is 0
+// (the cleared table), so no entry needs initialising: MAX holds v ^ 2^63, MIN holds ~(v ^ 2^63), both folded with
+// an unsigned atomicMax.
+#include "common.cuh"
+
+namespace {
+
+constexpr int F_THREADS = 256;
+constexpr int F_LEAD = 16;
+constexpr int F_OWN = 16384;
+constexpr int F_HALO = 4096;                      // longest line handled on the device, newline included
+constexpr int F_WIN = F_LEAD + F_OWN + F_HALO;    // 20496
+constexpr u32 F_G_MAX_PROBES = 1u << 14;
+constexpr u32 F_FB_MAXLEN = 0xFFFFu;             // the fallback list stores 16-bit lengths
+
+static_assert(F_WIN % 16 == 0, "window must be whole 16-byte vectors");
+static_assert(F_OWN % 16 == 0 && F_LEAD % 16 == 0, "tiles must keep 16-byte alignment");
+static_assert(TEXT_LEAD >= F_LEAD, "textbuf lead-in too small");
+static_assert(TEXT_TAIL_PAD >= F_WIN + 64, "textbuf tail pad too small");
+static_assert(TEXT_TAIL_PAD >= (int)F_FB_MAXLEN + 1, "tail pad must cover the long-line measurement");
+
+enum { S_ENTRIES = 0, S_LINES = 1, S_MAXABS = 2, S_FOLDED = 3, S_FLAGS = 4, S_LONG = 5, S_RAW = 6, S_FALLBACK = 7 };
+
+struct FieldsView {
+    u64 *keys;
+    u64 *counts;
+    u64 *reps;
+    u64 *stats;
+    u64 *fb;
+    u64 mask;
+    u64 seed;
+    u32 fb_cap;
+    u32 sep;
+    int key_field;
+    int val_field;   // DAMPR_FIELD_VAL_ONE: the constant 1
+    int key_int;
+    int op;
+    u32 cr_is_data;
+};
+
+struct SmemF {
+    alignas(16) u8 text[F_WIN];
+    u16 starts[F_OWN];
+    u32 warp_tot[F_THREADS / 32];
+    u32 nstarts;
+    u32 flags;
+};
+
+__device__ __forceinline__ u32 eq7(u32 x7, u32 k) {  // bit 7 of each byte set iff the (7-bit) byte == k
+    u32 z = x7 ^ (k * 0x01010101u);
+    return ~(z + 0x7F7F7F7Fu) & 0x80808080u;
+}
+
+// masks (bit 7 of each byte) of the 4 bytes of w: newline, separator, byte the device does not take
+__device__ __forceinline__ void classify(u32 w, u32 sep, bool cr_data, u32 &nl, u32 &sp, u32 &bad) {
+    const u32 hi = w & 0x80808080u;
+    const u32 x7 = w & 0x7F7F7F7Fu;
+    nl = eq7(x7, 0x0Au) & ~hi;
+    sp = eq7(x7, sep) & ~hi;
+    bad = hi | (eq7(x7, 0u) & ~hi);
+    if (!cr_data) bad |= eq7(x7, 0x0Du) & ~hi;
+}
+
+// parse [+-]?[0-9]{1,18} exactly; false for anything else (Python then decides)
+__device__ __forceinline__ bool parse_int(const u8 *p, u32 len, long long &out) {
+    u32 i = 0;
+    bool neg = false;
+    if (len && (p[0] == '+' || p[0] == '-')) {
+        neg = p[0] == '-';
+        i = 1;
+    }
+    const u32 nd = len - i;
+    if (nd == 0 || nd > 18) return false;
+    long long v = 0;
+    for (; i < len; ++i) {
+        const u32 d = (u32)p[i] - '0';
+        if (d > 9) return false;
+        v = v * 10 + d;
+    }
+    out = neg ? -v : v;
+    return true;
+}
+
+__device__ __forceinline__ u64 hash_bytes(const u8 *p, u32 len, u64 seed) {
+    u32 h1 = (u32)seed ^ 0x811C9DC5u, h2 = (u32)(seed >> 32) ^ 0x9747B28Cu;
+    for (u32 i = 0; i < len; ++i) {
+        const u32 v = p[i];
+        h1 = (h1 ^ v) * 16777619u;
+        h2 = (h2 ^ v) * 0x85EBCA6Bu + 0x9E3779B9u;
+        h2 = (h2 << 13) | (h2 >> 19);
+    }
+    return mix64((((u64)h1) << 32 | h2) ^ ((u64)len * 0x9E3779B97F4A7C15ULL)) | 0x8000000000000000ULL;
+}
+
+// fold (code -> value) into the global table; false if a hashed key's representative is a different string
+__device__ __forceinline__ bool fold_insert(const FieldsView &t, const u8 *text, u64 code, long long v, u64 rep,
+                                            u32 &flags) {
+    u64 slot = mix64(code) & t.mask;
+    for (u32 probe = 0; probe < F_G_MAX_PROBES; ++probe) {
+        u64 k = *((volatile u64 *)&t.keys[slot]);
+        if (k == 0) {
+            k = atomicCAS(&t.keys[slot], 0ULL, code);
+            if (k == 0) {
+                atomicAdd(&t.stats[S_ENTRIES], 1ULL);
+                k = code;
+            }
+        }
+        if (k == code) {
+            if (t.op == DAMPR_OP_SUM_I64) {
+                atomicAdd(&t.counts[slot], (u64)v);
+            } else {
+                const u64 ord = (u64)v ^ 0x8000000000000000ULL;
+                atomicMax(&t.counts[slot], t.op == DAMPR_OP_MAX_I64 ? ord : ~ord);
+            }
+            if (rep == ~0ULL) return true;
+            const u64 old = atomicMin(&t.reps[slot], rep);
+            if (old == ~0ULL || old == rep) return true;
+            const u32 len = (u32)(rep & 0xFFFFFu);
+            if ((u32)(old & 0xFFFFFu) != len) return false;
+            const u8 *a = text + (rep >> 20), *b = text + (old >> 20);
+            for (u32 i = 0; i < len; ++i)
+                if (a[i] != b[i]) return false;
+            return true;
+        }
+        slot = (slot + 1) & t.mask;
+    }
+    flags |= DAMPR_TF_TABLEFULL;
+    return true;
+}
+
+__global__ void __launch_bounds__(F_THREADS)
+text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    SmemF &s = *reinterpret_cast<SmemF *>(smem_raw);
+    const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
+    const bool cr_data = tab.cr_is_data != 0;
+    if (tid == 0) s.flags = 0;
+
+    u64 acc_lines = 0, acc_long = 0, acc_maxabs = 0;
+    u32 my_flags = 0;
+
+    for (u64 tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const u64 sgl = own_lo + tile * (u64)F_OWN;    // global offset of window position F_LEAD
+        const u32 own_len = (u32)min((u64)F_OWN, own_hi - sgl);
+        const u8 *gwin = text + sgl - F_LEAD;          // global address of window position 0
+        __syncthreads();                               // the previous tile's lines are done
+        {
+            const uint4 *src = reinterpret_cast<const uint4 *>(gwin);
+            uint4 *dst = reinterpret_cast<uint4 *>(s.text);
+            for (int i = tid; i < F_WIN / 16; i += F_THREADS) dst[i] = src[i];
+        }
+        __syncthreads();
+
+        // ---- line starts: x in [F_LEAD, F_LEAD + own_len) with a newline at x - 1, global offset < n --------
+        // thread t looks at the newlines in window bytes [F_LEAD + 64 t, +64) (starts one byte later); the start
+        // at F_LEAD itself (newline at F_LEAD - 1, or the lead-in of the text) is thread 0's
+        const u32 y0 = F_LEAD + 64 * tid;
+        const u32 hi = F_LEAD - 1 + own_len;        // newline positions y < hi give owned starts
+        u64 m = 0;
+        if (y0 < hi) {
+            const u32 *wp = reinterpret_cast<const u32 *>(s.text + y0);
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                const u32 w = wp[i];
+                const u32 nl = eq7(w & 0x7F7F7F7Fu, 0x0Au) & ~(w & 0x80808080u);
+                const u32 b4 = (((nl >> 7) & 0x01010101u) * 0x01020408u) >> 24;
+                m |= (u64)b4 << (4 * i);
+            }
+            if (y0 + 64 > hi) m &= (1ULL << (hi - y0)) - 1ULL;
+            const u64 gy0 = sgl - F_LEAD + y0;      // global offset of window byte y0
+            if (gy0 + 65 > n) {                     // start y0 + j + 1 must lie below n: j + 1 < n - gy0
+                const u64 lim = n > gy0 ? n - gy0 : 0;
+                m &= lim >= 1 ? ((1ULL << (lim - 1)) - 1ULL) : 0ULL;
+            }
+        }
+        const bool first = tid == 0 && s.text[F_LEAD - 1] == '\n' && sgl < n;
+        const u32 cnt = (u32)__popcll(m) + (first ? 1u : 0u);
+        u32 v = cnt;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const u32 o = __shfl_up_sync(0xFFFFFFFFu, v, d);
+            if ((int)lane >= d) v += o;
+        }
+        if (lane == 31) s.warp_tot[warp] = v;
+        __syncthreads();
+        if (warp == 0) {
+            u32 t = lane < F_THREADS / 32 ? s.warp_tot[lane] : 0u;
+            u32 x = t;
+#pragma unroll
+            for (int d = 1; d < F_THREADS / 32; d <<= 1) {
+                const u32 o = __shfl_up_sync(0xFFFFFFFFu, x, d);
+                if ((int)lane >= d) x += o;
+            }
+            if (lane < F_THREADS / 32) s.warp_tot[lane] = x - t;   // exclusive
+            if (lane == F_THREADS / 32 - 1) s.nstarts = x;
+        }
+        __syncthreads();
+        {
+            u32 ix = s.warp_tot[warp] + v - cnt;
+            if (first) s.starts[ix++] = (u16)F_LEAD;
+            while (m) {
+                const u32 j = (u32)__ffsll((long long)m) - 1u;
+                m &= m - 1;
+                s.starts[ix++] = (u16)(y0 + j + 1);
+            }
+        }
+        __syncthreads();
+
+        // ---- one line per thread -----------------------------------------------------------------------------
+        const u32 nst = s.nstarts;
+        for (u32 li = tid; li < nst; li += F_THREADS) {
+            const u32 q = s.starts[li];                       // window position of the first byte
+            const u32 lim = min(q + (u32)F_HALO, (u32)F_WIN);  // the line's newline must lie before lim
+            // pass 1: terminator, separators, bytes the device does not take
+            u32 p4 = q & ~3u;
+            u32 nsep = 0, end = 0xFFFFFFFFu;
+            bool bad = false;
+            u32 skip = q & 3u;
+            for (; p4 < lim; p4 += 4) {
+                const u32 w = *reinterpret_cast<const u32 *>(s.text + p4);
+                u32 nl, sp, bd;
+                classify(w, tab.sep, cr_data, nl, sp, bd);
+                if (skip) {
+                    const u32 keep = ~((1u << (8 * skip)) - 1u);
+                    nl &= keep;
+                    sp &= keep;
+                    bd &= keep;
+                    skip = 0;
+                }
+                if (nl) {
+                    const u32 b = ((u32)__ffs(nl) - 1u) >> 3;
+                    const u32 before = b ? ((1u << (8 * b)) - 1u) : 0u;
+                    nsep += (u32)__popc(sp & before);
+                    bad |= (bd & before) != 0;
+                    end = p4 + b;
+                    break;
+                }
+                nsep += (u32)__popc(sp);
+                bad |= bd != 0;
+            }
+            if (end >= lim) end = 0xFFFFFFFFu;   // the newline is at or past lim: not handled here
+            const u64 gq = sgl - F_LEAD + q;     // global offset of the line
+            bool to_host = bad || end == 0xFFFFFFFFu;
+            long long val = 1, kval = 0;
+            u64 code = 0, rep = ~0ULL;
+            if (!to_host) {
+                // resolve the field indices (Python semantics: negative counts from the end)
+                const int nf = (int)nsep + 1;
+                const int ki = tab.key_field < 0 ? tab.key_field + nf : tab.key_field;
+                const bool one = tab.val_field == DAMPR_FIELD_VAL_ONE;
+                const int vi = one ? 0 : (tab.val_field < 0 ? tab.val_field + nf : tab.val_field);
+                if (ki < 0 || ki >= nf || vi < 0 || vi >= nf) {
+                    to_host = true;   // IndexError: Python raises it
+                } else {
+                    // pass 2: field bounds (a separator at window position p closes field f and opens f + 1)
+                    u32 ks = (ki == 0) ? q : 0xFFFFFFFFu, ke = (ki == nf - 1) ? end : 0xFFFFFFFFu;
+                    u32 vs = (vi == 0) ? q : 0xFFFFFFFFu, ve = (vi == nf - 1) ? end : 0xFFFFFFFFu;
+                    const int need = max(ki, vi) + 1;   // separators to visit
+                    int f = 0;
+                    skip = q & 3u;
+                    for (p4 = q & ~3u; f < need && p4 < end; p4 += 4) {
+                        const u32 w = *reinterpret_cast<const u32 *>(s.text + p4);
+                        u32 nl, sp, bd;
+                        classify(w, tab.sep, cr_data, nl, sp, bd);
+                        if (skip) {
+                            sp &= ~((1u << (8 * skip)) - 1u);
+                            skip = 0;
+                        }
+                        while (sp && f < need) {
+                            const u32 p = p4 + (((u32)__ffs(sp) - 1u) >> 3);
+                            sp &= sp - 1;
+                            if (p >= end) break;
+                            if (f == ki) ke = p;
+                            if (f == vi) ve = p;
+                            ++f;
+                            if (f == ki) ks = p + 1;
+                            if (f == vi) vs = p + 1;
+                        }
+                    }
+                    const u32 klen = ke - ks;
+                    if (!one && !parse_int(s.text + vs, ve - vs, val)) to_host = true;
+                    if (!to_host) {
+                        if (tab.key_int) {
+                            if (!parse_int(s.text + ks, klen, kval)) to_host = true;
+                            else code = (u64)kval ^ 0x8000000000000000ULL;
+                        } else if (klen >= 1 && klen <= 9) {
+                            for (int i = (int)klen - 1; i >= 0; --i) code = (code << 7) | s.text[ks + i];
+                        } else {
+                            code = hash_bytes(s.text + ks, klen, tab.seed);
+                            rep = ((sgl - F_LEAD + ks) << 20) | klen;
+                            acc_long++;
+                        }
+                    }
+                }
+            }
+            if (to_host) {
+                // the host runs the stage's own functions on this line; a line longer than the device window is
+                // measured here (bytes up to own_hi + 64 KB are uploaded), one of 64 KB or more ends the scan
+                u32 len;
+                if (end != 0xFFFFFFFFu) {
+                    len = end - q;
+                } else {
+                    const u8 *g = text + gq;
+                    len = 0;
+                    while (len <= F_FB_MAXLEN && g[len] != '\n') ++len;
+                }
+                if (len > F_FB_MAXLEN) {
+                    my_flags |= DAMPR_TF_LONGLINE;
+                } else {
+                    const u64 ix = atomicAdd(&tab.stats[S_FALLBACK], 1ULL);
+                    if (ix < (u64)tab.fb_cap) tab.fb[ix] = (gq << 16) | (u64)len;
+                    else my_flags |= DAMPR_TF_NONASCII;
+                }
+                continue;
+            }
+            acc_lines++;
+            const u64 av = (u64)(val < 0 ? -val : val);
+            acc_maxabs = av > acc_maxabs ? av : acc_maxabs;
+            if (!fold_insert(tab, text, code, val, rep, my_flags)) my_flags |= DAMPR_TF_COLLISION;
+        }
+    }
+
+    // ---- publish counters ---------------------------------------------------------------------------------
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        acc_lines += __shfl_down_sync(0xFFFFFFFFu, acc_lines, d);
+        acc_long += __shfl_down_sync(0xFFFFFFFFu, acc_long, d);
+        const u64 o = __shfl_down_sync(0xFFFFFFFFu, acc_maxabs, d);
+        acc_maxabs = o > acc_maxabs ? o : acc_maxabs;
+    }
+    if (lane == 0) {
+        if (acc_lines) {
+            atomicAdd(&tab.stats[S_LINES], acc_lines);
+            atomicAdd(&tab.stats[S_FOLDED], acc_lines);
+        }
+        if (acc_long) atomicAdd(&tab.stats[S_LONG], acc_long);
+        if (acc_maxabs) atomicMax(&tab.stats[S_MAXABS], acc_maxabs);
+    }
+    if (my_flags) atomicOr(&s.flags, my_flags);
+    __syncthreads();
+    if (tid == 0 && s.flags) atomicOr(&tab.stats[S_FLAGS], (u64)s.flags);
+}
+
+}  // namespace
+
+extern "C" int32_t dampr_text_fields(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
+                                     uint64_t own_hi, const dampr_fields_spec *spec) {
+    ARG_CHECK(ctx, ctx && t && tb && spec, "null");
+    ARG_CHECK(ctx, own_lo <= own_hi && own_hi <= tb->n, "ownership range outside the text");
+    ARG_CHECK(ctx, (own_lo % 16) == 0, "own_lo must be a multiple of 16");
+    ARG_CHECK(ctx, spec->sep > 0 && spec->sep < 0x80 && spec->sep != '\n' && spec->sep != '\r',
+              "separator must be an ASCII byte other than NUL, '\\n' and '\\r'");
+    ARG_CHECK(ctx, spec->key_kind == DAMPR_FIELD_KEY_STR || spec->key_kind == DAMPR_FIELD_KEY_INT, "key kind");
+    ARG_CHECK(ctx, spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_MIN_I64 || spec->op == DAMPR_OP_MAX_I64,
+              "op must be DAMPR_OP_SUM_I64, DAMPR_OP_MIN_I64 or DAMPR_OP_MAX_I64");
+    if (own_hi <= own_lo) return DAMPR_OK;
+    const size_t smem = sizeof(SmemF);
+    CUDA_TRY(ctx, cudaFuncSetAttribute(text_fields_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
+    u64 grid = (u64)ctx->num_sms * 4;
+    if (grid > ntiles) grid = ntiles;
+    FieldsView tv{t->keys, t->counts, t->reps, t->stats, t->fb, t->cap - 1, 0x243F6A8885A308D3ULL, t->fb_cap,
+                  (u32)spec->sep, spec->key_field, spec->val_field, spec->key_kind == DAMPR_FIELD_KEY_INT ? 1 : 0,
+                  spec->op, spec->cr_is_data ? 1u : 0u};
+    wait_uploads(ctx);
+    {
+        ScopedTimer tm(ctx, DAMPR_K_TEXT_FIELDS);
+        text_fields_kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv);
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+    return DAMPR_OK;
+}

@@ -27,11 +27,32 @@ OP_SUM_I64, OP_SUM_F64, OP_COUNT, OP_MIN_I64, OP_MAX_I64, OP_MIN_F64, OP_MAX_F64
 # table flags
 TF_NONASCII, TF_CR, TF_LONGLINE, TF_TABLEFULL, TF_LONGTOKEN, TF_COLLISION = 1, 2, 4, 8, 16, 32
 TOK_FLAG_CR_DATA = 0x100
+# delimited-field scans (dampr_text_fields)
+FIELD_KEY_STR, FIELD_KEY_INT = 0, 1
+FIELD_VAL_ONE = 0x7FFFFFFF
+FIELDS_HALO = 65536
 
 KERNEL_NAMES = {
     1: "text_count", 2: "table_extract", 3: "text_verify", 4: "part_hist", 5: "part_scatter",
     6: "leaf_sort", 7: "seg_reduce", 8: "merge", 9: "join", 10: "probe", 11: "synth", 12: "misc",
+    13: "text_fields",
 }
+
+
+def decode_fold(acc, op):
+    """int64 values of a field scan's accumulators (uint64): MAX keeps v ^ 2^63, MIN ~(v ^ 2^63), SUM v"""
+    acc = np.asarray(acc, dtype=np.uint64)
+    if op == OP_MIN_I64:
+        acc = ~acc
+    if op in (OP_MIN_I64, OP_MAX_I64):
+        acc = acc ^ np.uint64(1 << 63)
+    return acc.view(np.int64)
+
+
+class FieldsSpec(C.Structure):
+    """dampr_fields_spec"""
+    _fields_ = [("sep", C.c_int32), ("key_field", C.c_int32), ("key_kind", C.c_int32), ("val_field", C.c_int32),
+                ("op", C.c_int32), ("cr_is_data", C.c_int32)]
 
 
 class DeviceError(RuntimeError):
@@ -92,6 +113,7 @@ def load_library():
     _sig(lib, "dampr_table_clear", vp, vp)
     _sig(lib, "dampr_text_count", vp, vp, vp, u64, u64, i32)
     _sig(lib, "dampr_text_verify", vp, vp, vp, u64, u64, i32)
+    _sig(lib, "dampr_text_fields", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec))
     _sig(lib, "dampr_table_stats", vp, vp, pu64)
     _sig(lib, "dampr_table_fallback_lines", vp, vp, vp, u64, pu64)
     _sig(lib, "dampr_table_fetch", vp, vp, vp, vp, vp, u64, pu64)
@@ -422,6 +444,24 @@ class Table(object):
         """cr_is_data: '\\r' is an ordinary byte (the reference's binary-mode .gz reader) instead of a line end"""
         m = int(mode) | (TOK_FLAG_CR_DATA if cr_is_data else 0)
         self.ctx.check(self.ctx.lib.dampr_text_count(self.ctx.h, self.h, tb.h, int(lo), int(hi), m))
+
+    def fields(self, tb, lo, hi, spec, cr_is_data=False):
+        """Fold the delimited fields of the lines starting in [lo, hi): spec = (sep byte, key field, key kind,
+        value field or FIELD_VAL_ONE, op); bytes up to hi + FIELDS_HALO must be uploaded."""
+        sep, kf, kind, vf, op = spec
+        s = FieldsSpec(int(sep), int(kf), int(kind), int(vf), int(op), 1 if cr_is_data else 0)
+        self.ctx.check(self.ctx.lib.dampr_text_fields(self.ctx.h, self.h, tb.h, int(lo), int(hi), C.byref(s)))
+
+    def fields_stats(self):
+        """stats() of a field scan under the names of its counters"""
+        st = self.stats()
+        return {"entries": st["entries"], "lines": st["lines"], "max_abs": st["empty"], "folded": st["folded"],
+                "flags": st["flags"], "hashed": st["hashed"], "fallback": st["fallback"]}
+
+    def fields_fetch(self, op):
+        """(codes, values int64) of a field scan: the accumulators decoded from their MIN / MAX codes"""
+        codes, acc, _reps = self.fetch()
+        return codes, decode_fold(acc, op)
 
     def fallback_lines(self):
         """uint64[]: (byte offset << 16) | length of every line the [^\\w]+ tokenisers handed back to the host"""

@@ -228,6 +228,70 @@ def tokenizer_mode(fn):
     return None
 
 
+FIELD_STR, FIELD_INT = "str", "int"
+
+
+def _split_sep(e):
+    """S if e is `x.split(S)` over the argument with a one-character ASCII separator other than '\\n', '\\r' and NUL
+    (the bytes that end or cannot appear in a device line), else None"""
+    if isinstance(e, E) and e.op == "call" and len(e.b) == 1 and isinstance(e.a, E) and e.a.op == "attr" \
+            and e.a.b == "split" and _is_arg(e.a.a):
+        ok, s = _const(e.b[0])
+        if ok and type(s) is str and len(s) == 1 and s.isascii() and s not in "\n\r\0":
+            return s
+    return None
+
+
+def _field_proj(e, record):
+    """(kind, i) if e is record(e')[i] (FIELD_STR) or int(record(e')[i]) (FIELD_INT) with a constant int i; record(x)
+    says whether x is the split record and returns its separator (any non-None value)"""
+    kind = FIELD_STR
+    if isinstance(e, E) and e.op == "call" and isinstance(e.a, E) and e.a.op == "obj" and e.a.a is int \
+            and len(e.b) == 1:
+        kind, e = FIELD_INT, e.b[0]
+    if not (isinstance(e, E) and e.op == "sub"):
+        return None
+    ok, i = _const(e.b)
+    if not ok or type(i) is not int or not -(1 << 30) <= i < (1 << 30):
+        return None
+    sep = record(e.a)
+    return None if sep is None else (kind, i, sep)
+
+
+def text_fields_spec(key_fn, value_fn, split_fn=None):
+    """Device field-scan spec of a keyed(key_fn, value_fn) over text lines, optionally behind map(split_fn):
+    (sep, key_index, key_kind, value_index) where the key is l.split(sep)[key_index] (FIELD_STR) or its int()
+    (FIELD_INT), and the value is int(l.split(sep)[value_index]), or the constant 1 when value_index is None.
+    Indices may be negative (Python's from-the-end). None for any other shape."""
+    fns = [f for f in (key_fn, value_fn, split_fn) if f is not None]
+    if not all(isinstance(f, types.FunctionType) and f.__code__.co_argcount == 1 for f in fns):
+        return None
+    ke, ve = analyze(key_fn), analyze(value_fn)
+    if ke is None or ve is None:
+        return None
+    if split_fn is None:
+        record = _split_sep                      # the split is inside the key / value functions
+    else:
+        sep = _split_sep(analyze(split_fn))
+        if sep is None:
+            return None
+
+        def record(x):                           # key / value functions index the split record
+            return sep if _is_arg(x) else None
+    k = _field_proj(ke, record)
+    if k is None:
+        return None
+    ok, one = _const(ve)
+    if ok:
+        if type(one) is not int or one != 1:
+            return None
+        return k[2], k[1], k[0], None
+    v = _field_proj(ve, record)
+    if v is None or v[0] != FIELD_INT or v[2] != k[2]:
+        return None
+    return k[2], k[1], k[0], v[1]
+
+
 def field_index(fn):
     """i if fn is `lambda x: x[i]` with a constant non-negative int i, else None."""
     e = analyze(fn)

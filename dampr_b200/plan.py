@@ -350,6 +350,8 @@ class TextScan(object):
     """One pass of the tokenise+combine kernel over a set of files (or a memory text), with the
     host->device copies pipelined against the kernel chunk by chunk."""
 
+    HALO = 16384   # bytes past a launch's range that must be uploaded before it (the kernel's window)
+
     def __init__(self, runner, sources, mode):
         self.runner = runner
         self.sources = sources
@@ -361,7 +363,12 @@ class TextScan(object):
         self.nbytes = 0
         self.has_cr = False   # '\r' seen: n_lines counts '\n' only and is not the universal-newline line count
 
-    def run(self):
+    def _launch(self, tab, tb, lo, hi):
+        """the kernel over the lines that start in [lo, hi)"""
+        tab.count(tb, lo, hi, self.mode, getattr(self, "_cr_is_data", False))
+
+    def _ingest(self):
+        """Upload the sources (or take the resident text), run _launch over all of it: (ctx, tb, table, stats)."""
         ctx = self.runner.ctx
         resident = len(self.sources) == 1 and self.sources[0][0] == "dev"
         tab = None
@@ -377,7 +384,8 @@ class TextScan(object):
             # files) does not apply when every source of the scan is a .gz file.
             if gz and len(gz) == len(self.sources):
                 self._cr_is_data = True
-            self._binary_src = [kind == "gz" for kind, _p in self.sources]
+            if not hasattr(self, "_binary_src"):   # (a repeated scan sees the inflated .gz sources as memory texts)
+                self._binary_src = [kind == "gz" for kind, _p in self.sources]
             if gz:
                 if dist.active():
                     raise NotLowerable("gzip inputs are not sharded across ranks")
@@ -392,15 +400,18 @@ class TextScan(object):
         # buffers are cached per context (see _cached_textbuf): nothing to release here
         if resident:
             self._tab = _cached_table(ctx)
-            self._tab.count(tb, 0, tb.n, self.mode, getattr(self, "_cr_is_data", False))
+            self._launch(self._tab, tb, 0, tb.n)
         else:
             self._upload_and_count(ctx, tb, sizes)
         tab = self._tab
         st = tab.stats()
-        flags = st["flags"]
         if getattr(self, "_cr_is_data", False):
-            flags &= ~dev.TF_CR
-            st = dict(st, flags=flags)
+            st = dict(st, flags=st["flags"] & ~dev.TF_CR)
+        return ctx, tb, tab, st
+
+    def run(self):
+        ctx, tb, tab, st = self._ingest()
+        flags = st["flags"]
         if dist.active():
             return self._finish_distributed(ctx, tb, tab, st)
         if (flags & dev.TF_TABLEFULL or st["entries"] * 2 > tab.capacity) and settings.text_table_log2 < 28 \
@@ -441,21 +452,7 @@ class TextScan(object):
             flags = tab.stats()["flags"]
         if flags & dev.TF_COLLISION:
             raise NotLowerable("64-bit key-code collision between two long tokens")
-        # keys are materialised on the device (K9) as fixed-width ASCII; only tokens longer than the
-        # width (rare) are patched on the host from their representative occurrence
-        # exact codes hold at most 12 characters: without hashed tokens 16 bytes per key are enough and
-        # neither codes nor representatives are needed on the host
-        hashed = bool(st["hashed"])
-        W = 32 if hashed else 16
-        words, counts, codes, reps = tab.fetch_words(tb, self.mode, W, with_codes=hashed)
-        too_long = np.flatnonzero(((codes >> np.uint64(63)) != 0) & ((reps & np.uint64(0xFFFFF)) > W)) if hashed else ()
-        if len(too_long):
-            wl = [b.decode("ascii") for b in words.tolist()]
-            for i in too_long.tolist():
-                rep = int(reps[i])
-                s = tb.download(rep >> 20, rep & 0xFFFFF).tobytes().decode("ascii")
-                wl[i] = s if self.mode == dev.TOK_WS else s.lower()
-            words = wl
+        words, counts = self._fetch_words(tab, tb, st, self.mode)
         self.words = words
         self.counts = counts.view(np.int64)
         self.n_lines = int(st["lines"])
@@ -469,21 +466,31 @@ class TextScan(object):
         self.host_lines = extra_lines
         return self
 
-    def _host_lines(self, tb, tab, st):
-        """Per-line fallback (SURVEY §8(a) T1/T2, VERDICT r1 #5): the lines the kernel could not tokenise the way
-        Python does — a non-ASCII byte (Unicode \\w and lower()), a '\\r' in a text-mode source (universal
-        newlines split the line) — were left out of the table; they are read back, split and tokenised here with
-        the reference's own rules (TextLineDataset.read dataset.py:458-476, the matched tokeniser idiom) and the
-        counts are merged. Returns ({token: count}, count of the '' token, number of lines)."""
-        if self.mode == dev.TOK_WS or not st.get("fallback"):
-            return {}, 0, 0
+    def _fetch_words(self, tab, tb, st, mode):
+        """(keys, counts) of the table: keys are materialised on the device (K9) as fixed-width ASCII; only tokens
+        longer than the width (rare) are patched on the host from their representative occurrence"""
+        # exact codes hold at most 12 characters: without hashed tokens 16 bytes per key are enough and
+        # neither codes nor representatives are needed on the host
+        hashed = bool(st["hashed"])
+        W = 32 if hashed else 16
+        words, counts, codes, reps = tab.fetch_words(tb, mode, W, with_codes=hashed)
+        too_long = np.flatnonzero(((codes >> np.uint64(63)) != 0) & ((reps & np.uint64(0xFFFFF)) > W)) if hashed else ()
+        if len(too_long):
+            wl = [b.decode("ascii") for b in words.tolist()]
+            for i in too_long.tolist():
+                rep = int(reps[i])
+                s = tb.download(rep >> 20, rep & 0xFFFFF).tobytes().decode("ascii")
+                wl[i] = s if mode == dev.TOK_WS else s.lower()
+            words = wl
+        return words, counts
+
+    def _fallback_lines(self, tb, tab):
+        """(offset, line) of every line on the table's fallback list, split by the reference's reader rules"""
         from .datasets import _iter_lines
         import bisect
         fb = np.sort(tab.fallback_lines())
         starts = getattr(self, "_layout_starts", None)
         binary = getattr(self, "_binary_src", None)
-        extra, empty, nlines = {}, 0, 0
-        dedup = self.mode == dev.TOK_NONWORD_LOWER_SET
         for e in fb.tolist():
             off, ln = e >> 16, e & 0xFFFF
             raw = tb.download(off, ln).tobytes()
@@ -492,14 +499,27 @@ class TextScan(object):
             universal = not getattr(self, "_cr_is_data", False)
             if starts and binary and len(binary) == len(starts):
                 universal = not binary[max(0, bisect.bisect_right(starts, off) - 1)]
-            for _o, line in _iter_lines(raw, off, universal=universal):
-                nlines += 1
-                toks = _NONWORD_RX.split(line.lower())
-                for t in (set(toks) if dedup else toks):
-                    if t == "":
-                        empty += 1
-                    else:
-                        extra[t] = extra.get(t, 0) + 1
+            for item in _iter_lines(raw, off, universal=universal):
+                yield item
+
+    def _host_lines(self, tb, tab, st):
+        """Per-line fallback (SURVEY §8(a) T1/T2, VERDICT r1 #5): the lines the kernel could not tokenise the way
+        Python does — a non-ASCII byte (Unicode \\w and lower()), a '\\r' in a text-mode source (universal
+        newlines split the line) — were left out of the table; they are read back, split and tokenised here with
+        the reference's own rules (TextLineDataset.read dataset.py:458-476, the matched tokeniser idiom) and the
+        counts are merged. Returns ({token: count}, count of the '' token, number of lines)."""
+        if self.mode == dev.TOK_WS or not st.get("fallback"):
+            return {}, 0, 0
+        extra, empty, nlines = {}, 0, 0
+        dedup = self.mode == dev.TOK_NONWORD_LOWER_SET
+        for _o, line in self._fallback_lines(tb, tab):
+            nlines += 1
+            toks = _NONWORD_RX.split(line.lower())
+            for t in (set(toks) if dedup else toks):
+                if t == "":
+                    empty += 1
+                else:
+                    extra[t] = extra.get(t, 0) + 1
         return extra, empty, nlines
 
     def _finish_distributed(self, ctx, tb, tab, st):
@@ -646,12 +666,12 @@ class TextScan(object):
 
     def _count_ready(self, tab, tb, counted, done, total, final):
         """Launch the kernel over every 4 KB-aligned range whose halo has been uploaded."""
-        HALO = 16384
+        HALO = self.HALO
         hi = total if final else max(counted, ((done - HALO) // 4096) * 4096 if done > HALO else 0)
         if hi > counted:
             a, b = max(counted, self._own[0]), min(hi, self._own[1])
             if b > a:
-                tab.count(tb, a, b, self.mode, getattr(self, "_cr_is_data", False))
+                self._launch(tab, tb, a, b)
             counted = hi
         self._counted = counted
         return counted
@@ -666,6 +686,109 @@ class TextScan(object):
             tb.upload_file(base + off, path, off, ln)
             off += ln
             self._count_ready(tab, tb, self._counted, base + off, total, final=False)
+
+
+class FieldScan(TextScan):
+    """One pass of the delimited-field kernel (dampr_text_fields) over a text input: TextScan's ingest with the field
+    fold as the per-range launch. The lines the device hands back go through the stage's own functions."""
+
+    HALO = dev.FIELDS_HALO   # a line longer than the kernel's window is measured up to 64 KB past its start
+
+    def __init__(self, runner, sources, spec, op, stage):
+        TextScan.__init__(self, runner, sources, None)
+        self.spec = spec     # (separator byte, key index, key kind, value index or FIELD_VAL_ONE)
+        self.op = op
+        self.stage = stage
+        self.keys = self.values = None
+        self.groups = self.host_lines = 0
+
+    def _launch(self, tab, tb, lo, hi):
+        tab.fields(tb, lo, hi, tuple(self.spec) + (self.op,), getattr(self, "_cr_is_data", False))
+
+    def run(self):
+        _ctx, tb, tab, _st = self._ingest()
+        st = tab.fields_stats()
+        flags = st["flags"]
+        if (flags & dev.TF_TABLEFULL or st["entries"] * 2 > tab.capacity) and settings.text_table_log2 < 28 \
+                and not resident_retry_block(self):
+            settings.text_table_log2 = int(settings.text_table_log2) + 2   # as TextScan.run: a 4x table, scan again
+            return self.run()
+        if flags & dev.TF_TABLEFULL:
+            raise NotLowerable("combiner table overflow")
+        if flags & (dev.TF_NONASCII | dev.TF_LONGLINE):
+            raise NotLowerable("more lines for the host than the fallback list holds, or a line of 64 KB or more")
+        if flags & dev.TF_COLLISION:
+            raise NotLowerable("64-bit key-code collision between two long keys")
+        if self.spec[2] == dev.FIELD_KEY_INT:
+            codes, acc, _reps = tab.fetch()
+            keys = (codes ^ np.uint64(1 << 63)).view(np.int64)
+        else:
+            keys, acc = self._fetch_words(tab, tb, st, dev.TOK_WS)   # 7-bit codes: the str.split decoding
+        vals = dev.decode_fold(acc, self.op)
+        # the lines the device handed back: the stage's own mapper functions, folded with its binop
+        binop = self.stage.options.get("binop")
+        extra, nrec, max_abs = {}, 0, 0
+        if st["fallback"]:
+            it = iter(self._fallback_lines(tb, tab))
+            for p in _parts(self.stage.mapper):
+                it = p.stream(it)
+            for k, v in it:
+                nrec += 1
+                max_abs = max(max_abs, abs(v))
+                extra[k] = binop(extra[k], v) if k in extra else v
+        # Python's ints are unbounded, the table's are 64-bit (SURVEY B12): the bound of _may_overflow
+        if self.op == dev.OP_SUM_I64 and (int(st["folded"]) + nrec) * max(int(st["max_abs"]), max_abs) >= (1 << 62):
+            raise NotLowerable("64-bit sum could overflow (SURVEY B12)")
+        self.keys, self.values = _merge_folds(keys, vals, extra, binop)
+        self.groups = len(self.values)
+        self.n_lines = int(st["lines"]) + nrec   # one record per line
+        self.host_lines = nrec
+        return self
+
+
+def _merge_folds(keys, vals, extra, binop):
+    """(keys, int64 values) of a device fold plus {key: value} folded on the host: a key present in both gets
+    binop(device value, host value). `keys` is an 'S' array, an int64 array or a list of str."""
+    if not extra:
+        return keys, vals
+    if any(not -(1 << 63) <= v < (1 << 63) for v in extra.values()) or \
+            any(type(k) is int and not -(1 << 63) <= k < (1 << 63) for k in extra):
+        raise NotLowerable("a host-folded value or key outside int64")
+    vals = np.array(vals, dtype=np.int64, copy=True)
+    if isinstance(keys, np.ndarray) and keys.dtype.kind == "S":
+        W = keys.dtype.itemsize
+        fit = [k for k in extra if type(k) is str and k.isascii() and len(k) <= W and "\0" not in k]
+        probe = np.array([k.encode("ascii") for k in fit], dtype=keys.dtype)
+        hit = np.flatnonzero(np.isin(keys, probe)) if fit and len(keys) else np.zeros(0, dtype=np.int64)
+        pos = {b.decode("ascii"): i for b, i in zip(keys[hit].tolist(), hit.tolist())}
+    elif isinstance(keys, np.ndarray):
+        fit = [k for k in extra if type(k) is int]
+        probe = np.array(fit, dtype=np.int64)
+        hit = np.flatnonzero(np.isin(keys, probe)) if fit and len(keys) else np.zeros(0, dtype=np.int64)
+        pos = dict(zip(keys[hit].tolist(), hit.tolist()))
+    else:
+        pos = {k: i for i, k in enumerate(keys)}
+    new = []
+    for k, v in extra.items():
+        i = pos.get(k) if type(k) in (str, int) else None
+        if i is None:
+            new.append(k)
+            continue
+        r = binop(int(vals[i]), v)
+        if not -(1 << 63) <= r < (1 << 63):
+            raise NotLowerable("a merged value outside int64")
+        vals[i] = r
+    if not new:
+        return keys, vals
+    nv = np.array([extra[k] for k in new], dtype=np.int64)
+    if isinstance(keys, np.ndarray) and keys.dtype.kind == "S" and \
+            all(type(k) is str and k.isascii() and len(k) <= keys.dtype.itemsize and "\0" not in k for k in new):
+        keys = np.concatenate((keys, np.array([k.encode("ascii") for k in new], dtype=keys.dtype)))
+    elif isinstance(keys, np.ndarray) and keys.dtype.kind == "i" and all(type(k) is int for k in new):
+        keys = np.concatenate((keys, np.array(new, dtype=np.int64)))
+    else:
+        keys = Frame._pylist(keys) + new
+    return keys, np.concatenate((vals, nv))
 
 
 def _source_key(sources):
@@ -723,6 +846,31 @@ def _match_text_count(stage, inputs):
     if lowering.binop_kind(stage.options.get("binop")) != lowering.ADD:
         return None
     return src, mode
+
+
+def _match_text_fields(stage, inputs):
+    """[map(l.split(S)) ->] keyed(field key, 1 | int(field)) + PartialReduceCombiner(+ | min | max) over text:
+    (sources, (sep byte, key index, key kind, value index or FIELD_VAL_ONE), op) or None"""
+    if not isinstance(stage, GMap) or len(inputs) != 1:
+        return None
+    src = _text_files(inputs[0])
+    if src is None:
+        return None
+    ks = _opkinds(stage.mapper)
+    if ks is None or [k for k, _ in ks] not in (["keyed"], ["map", "keyed"]):
+        return None
+    if not isinstance(stage.combiner, ops.PartialReduceCombiner):
+        return None
+    kind = lowering.binop_kind(stage.options.get("binop"))
+    if kind not in (lowering.ADD, lowering.MIN, lowering.MAX):
+        return None
+    keyed = ks[-1][1]
+    spec = lowering.text_fields_spec(keyed.fn, keyed.fn2, ks[0][1].fn if len(ks) == 2 else None)
+    if spec is None:
+        return None
+    sep, ki, kkind, vi = spec
+    return src, (ord(sep), ki, dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR,
+                 dev.FIELD_VAL_ONE if vi is None else vi), _FOLD_OPS[kind]
 
 
 def _match_line_count(stage, inputs):
@@ -791,6 +939,16 @@ def _lower_map(runner, stage, inputs, si):
         runner.stats.add(stage, "device text tokenise+combine",
                          "bytes=%d terms=%d lines=%d" % (scan.nbytes, len(words), scan.n_lines))
         return f
+    m = _match_text_fields(stage, inputs)
+    if m is not None:
+        if dist.active():
+            raise NotLowerable("the field scan runs on one process")
+        src, spec, op = m
+        scan = FieldScan(runner, src, spec, op, stage).run()
+        runner.stats.add(stage, "device text fields scan+combine",
+                         "bytes=%d lines=%d groups=%d host_lines=%d" % (scan.nbytes, scan.n_lines, scan.groups,
+                                                                        scan.host_lines))
+        return Frame(scan.keys, [scan.values], scalar=True, combined=True)
     if _match_line_count(stage, inputs):
         ds = inputs[0]
         src = _text_files(ds)
