@@ -23,7 +23,7 @@ def build(force=False, verbose=False):
     nvcc = os.environ.get("NVCC") or shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
     objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
-    deps = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "leaf.cuh"), os.path.join(HERE, "..", "include", "dampr_b200.h")]
+    deps = [os.path.join(CSRC, f) for f in ("common.cuh", "leaf.cuh", "fparse.cuh", "pow5.cuh")] + [os.path.join(HERE, "..", "include", "dampr_b200.h")]
     objs = []
     relink = force or not os.path.exists(LIB)
     for src in SOURCES:

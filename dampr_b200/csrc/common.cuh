@@ -103,6 +103,8 @@ struct dampr_table {
     u32 fb_cap;
     u32 cap_log2;
     u64 cap;
+    u64 *tiles;   // device: per-tile line counts / bases of dampr_text_fields_records (grown on demand)
+    u64 tiles_cap;
 };
 
 struct dampr_kv {

@@ -1,5 +1,6 @@
 // fields.cu — delimited-field scan + combine: `line.split(sep)[i]` keys folded with a count, an int sum, a minimum
-// or a maximum of `int(line.split(sep)[j])`.
+// or a maximum of `int(line.split(sep)[j])`, a minimum or maximum of `float(line.split(sep)[j])`, and the per-line
+// records of float sums and mean().
 //
 // Replaces, for the lowered field idioms, the reference's per-record Python in the map stage:
 //   TextLineDataset.read      dampr/dataset.py:458-476  (line ownership, '\n' stripping)
@@ -22,8 +23,18 @@
 //
 // Accumulators: SUM adds two's-complement values. MIN and MAX keep an order-preserving code whose identity is 0
 // (the cleared table), so no entry needs initialising: MAX holds v ^ 2^63, MIN holds ~(v ^ 2^63), both folded with
-// an unsigned atomicMax.
+// an unsigned atomicMax. `float()` values (fparse.cuh) under MIN / MAX use the order-preserving code of the double,
+// bits ^ (sign ? ~0 : 2^63), the same way.
+//
+// Record mode (float sums, mean()): float + is not associative bit for bit, so the values are not folded here.
+// The kernel writes one 16-byte record {key code, value bits} per owned line, in line order, for a sort + ordered
+// segmented reduce on the caller's side; the table still takes one insert per line and counts the lines of each
+// key. The record index of a line is run_base + tile_base + its index among the tile's line starts. A count pass
+// (the same kernel, COUNT mode, sharing the line-start code) writes the lines per tile, one CTA scans them into
+// tile bases and advances run_base (a table stats slot), then the fold pass writes the records. No CTA waits for
+// another, and the records of a scan do not depend on how it is cut into ranges.
 #include "common.cuh"
+#include "fparse.cuh"
 
 namespace {
 
@@ -41,7 +52,18 @@ static_assert(TEXT_LEAD >= F_LEAD, "textbuf lead-in too small");
 static_assert(TEXT_TAIL_PAD >= F_WIN + 64, "textbuf tail pad too small");
 static_assert(TEXT_TAIL_PAD >= (int)F_FB_MAXLEN + 1, "tail pad must cover the long-line measurement");
 
-enum { S_ENTRIES = 0, S_LINES = 1, S_MAXABS = 2, S_FOLDED = 3, S_FLAGS = 4, S_LONG = 5, S_RAW = 6, S_FALLBACK = 7 };
+// S_RECORDS: record mode's running record count (run_base of the next range)
+enum { S_ENTRIES = 0, S_LINES = 1, S_MAXABS = 2, S_FOLDED = 3, S_FLAGS = 4, S_LONG = 5, S_RECORDS = 6, S_FALLBACK = 7 };
+
+enum { VK_INT = 0, VK_F64 = 1 };                      // value kind: int() or float()
+enum { M_TABLE = 0, M_COUNT = 1, M_RECORDS = 2 };     // fold into the table / count lines per tile / write records
+constexpr int SCAN_THREADS = 1024;
+
+struct RecView {
+    ulonglong2 *rec;
+    u64 cap;
+    u64 *tiles;   // M_COUNT: lines per tile (written); M_RECORDS: record index of each tile's first line (read)
+};
 
 struct FieldsView {
     u64 *keys;
@@ -114,7 +136,9 @@ __device__ __forceinline__ u64 hash_bytes(const u8 *p, u32 len, u64 seed) {
     return mix64((((u64)h1) << 32 | h2) ^ ((u64)len * 0x9E3779B97F4A7C15ULL)) | 0x8000000000000000ULL;
 }
 
-// fold (code -> value) into the global table; false if a hashed key's representative is a different string
+// fold (code -> value) into the global table; false if a hashed key's representative is a different string.
+// F64: v holds the bits of a double (MIN / MAX only)
+template <bool F64>
 __device__ __forceinline__ bool fold_insert(const FieldsView &t, const u8 *text, u64 code, long long v, u64 rep,
                                             u32 &flags) {
     u64 slot = mix64(code) & t.mask;
@@ -128,7 +152,10 @@ __device__ __forceinline__ bool fold_insert(const FieldsView &t, const u8 *text,
             }
         }
         if (k == code) {
-            if (t.op == DAMPR_OP_SUM_I64) {
+            if constexpr (F64) {
+                const u64 ord = (u64)v ^ (v < 0 ? ~0ULL : 0x8000000000000000ULL);
+                atomicMax(&t.counts[slot], t.op == DAMPR_OP_MAX_F64 ? ord : ~ord);
+            } else if (t.op == DAMPR_OP_SUM_I64) {
                 atomicAdd(&t.counts[slot], (u64)v);
             } else {
                 const u64 ord = (u64)v ^ 0x8000000000000000ULL;
@@ -150,8 +177,52 @@ __device__ __forceinline__ bool fold_insert(const FieldsView &t, const u8 *text,
     return true;
 }
 
+__device__ __forceinline__ void put_record(const RecView &rv, u64 ix, u64 code, u64 bits, u32 &flags) {
+    if (ix < rv.cap) rv.rec[ix] = make_ulonglong2(code, bits);
+    else flags |= DAMPR_TF_RECFULL;
+}
+
+// lines per tile -> record index of each tile's first line (exclusive scan from the running count, which
+// advances by the range's lines): one CTA, no inter-CTA waiting
+__global__ void __launch_bounds__(SCAN_THREADS) fields_tile_scan_kernel(u64 *tiles, u64 ntiles, u64 *run) {
+    __shared__ u64 warp_tot[SCAN_THREADS / 32];
+    __shared__ u64 carry;
+    const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) carry = *run;
+    __syncthreads();
+    for (u64 b = 0; b < ntiles; b += SCAN_THREADS) {
+        const u64 i = b + tid;
+        const u64 c = i < ntiles ? tiles[i] : 0;
+        u64 v = c;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const u64 o = __shfl_up_sync(0xFFFFFFFFu, v, d);
+            if ((int)lane >= d) v += o;
+        }
+        if (lane == 31) warp_tot[warp] = v;
+        __syncthreads();
+        if (warp == 0) {
+            const u64 t = warp_tot[lane];
+            u64 x = t;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const u64 o = __shfl_up_sync(0xFFFFFFFFu, x, d);
+                if ((int)lane >= d) x += o;
+            }
+            warp_tot[lane] = x - t;   // exclusive
+        }
+        __syncthreads();
+        if (i < ntiles) tiles[i] = carry + warp_tot[warp] + v - c;
+        __syncthreads();
+        if (tid == SCAN_THREADS - 1) carry += warp_tot[warp] + v;
+        __syncthreads();
+    }
+    if (tid == 0) *run = carry;
+}
+
+template <int VK, int MODE>
 __global__ void __launch_bounds__(F_THREADS)
-text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab) {
+text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SmemF &s = *reinterpret_cast<SmemF *>(smem_raw);
     const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -218,6 +289,10 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
             if (lane == F_THREADS / 32 - 1) s.nstarts = x;
         }
         __syncthreads();
+        if constexpr (MODE == M_COUNT) {
+            if (tid == 0) rv.tiles[tile] = s.nstarts;
+            continue;
+        }
         {
             u32 ix = s.warp_tot[warp] + v - cnt;
             if (first) s.starts[ix++] = (u16)F_LEAD;
@@ -231,6 +306,7 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
 
         // ---- one line per thread -----------------------------------------------------------------------------
         const u32 nst = s.nstarts;
+        const u64 tbase = MODE == M_RECORDS ? rv.tiles[tile] : 0;
         for (u32 li = tid; li < nst; li += F_THREADS) {
             const u32 q = s.starts[li];                       // window position of the first byte
             const u32 lim = min(q + (u32)F_HALO, (u32)F_WIN);  // the line's newline must lie before lim
@@ -301,7 +377,13 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
                         }
                     }
                     const u32 klen = ke - ks;
-                    if (!one && !parse_int(s.text + vs, ve - vs, val)) to_host = true;
+                    if constexpr (VK == VK_F64) {
+                        double d;
+                        if (parse_f64(s.text + vs, ve - vs, d)) val = __double_as_longlong(d);
+                        else to_host = true;
+                    } else if (!one && !parse_int(s.text + vs, ve - vs, val)) {
+                        to_host = true;
+                    }
                     if (!to_host) {
                         if (tab.key_int) {
                             if (!parse_int(s.text + ks, klen, kval)) to_host = true;
@@ -334,12 +416,24 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
                     if (ix < (u64)tab.fb_cap) tab.fb[ix] = (gq << 16) | (u64)len;
                     else my_flags |= DAMPR_TF_NONASCII;
                 }
+                if constexpr (MODE == M_RECORDS) put_record(rv, tbase + li, 0, 0, my_flags);   // a hole
                 continue;
             }
             acc_lines++;
-            const u64 av = (u64)(val < 0 ? -val : val);
-            acc_maxabs = av > acc_maxabs ? av : acc_maxabs;
-            if (!fold_insert(tab, text, code, val, rep, my_flags)) my_flags |= DAMPR_TF_COLLISION;
+            if constexpr (VK == VK_INT) {
+                const u64 av = (u64)(val < 0 ? -val : val);
+                acc_maxabs = av > acc_maxabs ? av : acc_maxabs;
+            } else if ((u64)val == 0x8000000000000000ULL) {
+                my_flags |= DAMPR_TF_NEGZERO;
+            }
+            bool same;
+            if constexpr (MODE == M_RECORDS) {
+                put_record(rv, tbase + li, code, (u64)val, my_flags);
+                same = fold_insert<false>(tab, text, code, 1, rep, my_flags);   // the line count of the key
+            } else {
+                same = fold_insert<VK == VK_F64>(tab, text, code, val, rep, my_flags);
+            }
+            if (!same) my_flags |= DAMPR_TF_COLLISION;
         }
     }
 
@@ -364,32 +458,86 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
     if (tid == 0 && s.flags) atomicOr(&tab.stats[S_FLAGS], (u64)s.flags);
 }
 
-}  // namespace
+// one kernel over the tiles of [own_lo, own_hi)
+template <int VK, int MODE>
+int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const FieldsView &tv, const RecView &rv,
+                  int timer) {
+    const size_t smem = sizeof(SmemF);
+    CUDA_TRY(ctx, cudaFuncSetAttribute(text_fields_kernel<VK, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)smem));
+    const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
+    u64 grid = (u64)ctx->num_sms * 4;
+    if (grid > ntiles) grid = ntiles;
+    {
+        ScopedTimer tm(ctx, timer);
+        text_fields_kernel<VK, MODE><<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi,
+                                                                                        tv, rv);
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+    return DAMPR_OK;
+}
 
-extern "C" int32_t dampr_text_fields(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
-                                     uint64_t own_hi, const dampr_fields_spec *spec) {
+int check_fields_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own_lo, u64 own_hi,
+                      const dampr_fields_spec *spec) {
     ARG_CHECK(ctx, ctx && t && tb && spec, "null");
     ARG_CHECK(ctx, own_lo <= own_hi && own_hi <= tb->n, "ownership range outside the text");
     ARG_CHECK(ctx, (own_lo % 16) == 0, "own_lo must be a multiple of 16");
     ARG_CHECK(ctx, spec->sep > 0 && spec->sep < 0x80 && spec->sep != '\n' && spec->sep != '\r',
               "separator must be an ASCII byte other than NUL, '\\n' and '\\r'");
     ARG_CHECK(ctx, spec->key_kind == DAMPR_FIELD_KEY_STR || spec->key_kind == DAMPR_FIELD_KEY_INT, "key kind");
-    ARG_CHECK(ctx, spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_MIN_I64 || spec->op == DAMPR_OP_MAX_I64,
-              "op must be DAMPR_OP_SUM_I64, DAMPR_OP_MIN_I64 or DAMPR_OP_MAX_I64");
+    return DAMPR_OK;
+}
+
+FieldsView fields_view(dampr_table *t, const dampr_fields_spec *spec, int op) {
+    return FieldsView{t->keys, t->counts, t->reps, t->stats, t->fb, t->cap - 1, 0x243F6A8885A308D3ULL, t->fb_cap,
+                      (u32)spec->sep, spec->key_field, spec->val_field, spec->key_kind == DAMPR_FIELD_KEY_INT ? 1 : 0,
+                      op, spec->cr_is_data ? 1u : 0u};
+}
+
+}  // namespace
+
+extern "C" int32_t dampr_text_fields(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
+                                     uint64_t own_hi, const dampr_fields_spec *spec) {
+    if (int r = check_fields_args(ctx, t, tb, own_lo, own_hi, spec)) return r;
+    const bool f64 = spec->op == DAMPR_OP_MIN_F64 || spec->op == DAMPR_OP_MAX_F64;
+    ARG_CHECK(ctx, f64 || spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_MIN_I64 ||
+                       spec->op == DAMPR_OP_MAX_I64,
+              "op must be DAMPR_OP_SUM_I64, DAMPR_OP_MIN_I64, DAMPR_OP_MAX_I64, DAMPR_OP_MIN_F64 or DAMPR_OP_MAX_F64");
+    ARG_CHECK(ctx, !f64 || spec->val_field != DAMPR_FIELD_VAL_ONE, "a float op needs a value field");
     if (own_hi <= own_lo) return DAMPR_OK;
-    const size_t smem = sizeof(SmemF);
-    CUDA_TRY(ctx, cudaFuncSetAttribute(text_fields_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
-    u64 grid = (u64)ctx->num_sms * 4;
-    if (grid > ntiles) grid = ntiles;
-    FieldsView tv{t->keys, t->counts, t->reps, t->stats, t->fb, t->cap - 1, 0x243F6A8885A308D3ULL, t->fb_cap,
-                  (u32)spec->sep, spec->key_field, spec->val_field, spec->key_kind == DAMPR_FIELD_KEY_INT ? 1 : 0,
-                  spec->op, spec->cr_is_data ? 1u : 0u};
+    const FieldsView tv = fields_view(t, spec, spec->op);
     wait_uploads(ctx);
+    if (f64) return launch_fields<VK_F64, M_TABLE>(ctx, tb, own_lo, own_hi, tv, RecView{}, DAMPR_K_TEXT_FIELDS);
+    return launch_fields<VK_INT, M_TABLE>(ctx, tb, own_lo, own_hi, tv, RecView{}, DAMPR_K_TEXT_FIELDS);
+}
+
+extern "C" int32_t dampr_text_fields_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
+                                             uint64_t own_hi, const dampr_fields_spec *spec, dampr_kv *rec) {
+    if (int r = check_fields_args(ctx, t, tb, own_lo, own_hi, spec)) return r;
+    ARG_CHECK(ctx, rec != nullptr, "null");
+    ARG_CHECK(ctx, spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_SUM_F64,
+              "op must be DAMPR_OP_SUM_I64 or DAMPR_OP_SUM_F64");
+    ARG_CHECK(ctx, spec->val_field != DAMPR_FIELD_VAL_ONE, "record mode needs a value field");
+    if (own_hi <= own_lo) return DAMPR_OK;
+    const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
+    if (ntiles > t->tiles_cap) {
+        CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));   // the previous range may still read the old array
+        cudaFree(t->tiles);
+        t->tiles = nullptr;
+        t->tiles_cap = 0;
+        CUDA_TRY(ctx, cudaMalloc(&t->tiles, ntiles * sizeof(u64)));
+        t->tiles_cap = ntiles;
+    }
+    const FieldsView tv = fields_view(t, spec, DAMPR_OP_SUM_I64);   // the table counts the lines of each key
+    const RecView rv{rec->rec, rec->capacity, t->tiles};
+    wait_uploads(ctx);
+    if (int r = launch_fields<VK_INT, M_COUNT>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS_COUNT)) return r;
     {
-        ScopedTimer tm(ctx, DAMPR_K_TEXT_FIELDS);
-        text_fields_kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv);
+        ScopedTimer tm(ctx, DAMPR_K_TEXT_FIELDS_COUNT);
+        fields_tile_scan_kernel<<<1, SCAN_THREADS, 0, ctx->stream>>>(t->tiles, ntiles, t->stats + S_RECORDS);
     }
     CUDA_TRY(ctx, cudaGetLastError());
-    return DAMPR_OK;
+    if (spec->op == DAMPR_OP_SUM_F64)
+        return launch_fields<VK_F64, M_RECORDS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS);
+    return launch_fields<VK_INT, M_RECORDS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS);
 }

@@ -652,7 +652,7 @@ int32_t dampr_table_create(dampr_ctx *ctx, uint32_t capacity_log2, dampr_table *
     dampr_table *t = new dampr_table();
     t->cap_log2 = capacity_log2;
     t->cap = 1ULL << capacity_log2;
-    t->keys = t->counts = t->reps = t->stats = t->fb = nullptr;
+    t->keys = t->counts = t->reps = t->stats = t->fb = t->tiles = nullptr;
     t->fb_cap = 1u << 16;
     if (cudaMalloc(&t->keys, t->cap * 8) != cudaSuccess || cudaMalloc(&t->counts, t->cap * 8) != cudaSuccess ||
         cudaMalloc(&t->reps, t->cap * 8) != cudaSuccess || cudaMalloc(&t->stats, 8 * 8) != cudaSuccess ||
@@ -682,6 +682,7 @@ int32_t dampr_table_destroy(dampr_ctx *ctx, dampr_table *t) {
     cudaFree(t->reps);
     cudaFree(t->stats);
     cudaFree(t->fb);
+    cudaFree(t->tiles);
     delete t;
     return DAMPR_OK;
 }

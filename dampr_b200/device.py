@@ -26,6 +26,7 @@ KEY_RAW, KEY_MIX, KEY_I64, KEY_F64 = 0, 1, 2, 3
 OP_SUM_I64, OP_SUM_F64, OP_COUNT, OP_MIN_I64, OP_MAX_I64, OP_MIN_F64, OP_MAX_F64, OP_FIRST, OP_LAST = range(9)
 # table flags
 TF_NONASCII, TF_CR, TF_LONGLINE, TF_TABLEFULL, TF_LONGTOKEN, TF_COLLISION = 1, 2, 4, 8, 16, 32
+TF_RECFULL, TF_NEGZERO = 64, 128   # field scans: record buffer full / a float() field parsed to -0.0
 TOK_FLAG_CR_DATA = 0x100
 # delimited-field scans (dampr_text_fields)
 FIELD_KEY_STR, FIELD_KEY_INT = 0, 1
@@ -35,13 +36,17 @@ FIELDS_HALO = 65536
 KERNEL_NAMES = {
     1: "text_count", 2: "table_extract", 3: "text_verify", 4: "part_hist", 5: "part_scatter",
     6: "leaf_sort", 7: "seg_reduce", 8: "merge", 9: "join", 10: "probe", 11: "synth", 12: "misc",
-    13: "text_fields",
+    13: "text_fields", 14: "text_fields_count",
 }
 
 
 def decode_fold(acc, op):
-    """int64 values of a field scan's accumulators (uint64): MAX keeps v ^ 2^63, MIN ~(v ^ 2^63), SUM v"""
+    """int64 values of a field scan's accumulators (uint64): MAX keeps v ^ 2^63, MIN ~(v ^ 2^63), SUM v; float64
+    values under MIN_F64 / MAX_F64, whose codes are bits ^ (sign ? ~0 : 2^63) (MIN: the complement)"""
     acc = np.asarray(acc, dtype=np.uint64)
+    if op in (OP_MIN_F64, OP_MAX_F64):
+        c = ~acc if op == OP_MIN_F64 else acc
+        return np.where(c >> np.uint64(63) != 0, c ^ np.uint64(1 << 63), ~c).view(np.float64)
     if op == OP_MIN_I64:
         acc = ~acc
     if op in (OP_MIN_I64, OP_MAX_I64):
@@ -114,6 +119,7 @@ def load_library():
     _sig(lib, "dampr_text_count", vp, vp, vp, u64, u64, i32)
     _sig(lib, "dampr_text_verify", vp, vp, vp, u64, u64, i32)
     _sig(lib, "dampr_text_fields", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec))
+    _sig(lib, "dampr_text_fields_records", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), vp)
     _sig(lib, "dampr_table_stats", vp, vp, pu64)
     _sig(lib, "dampr_table_fallback_lines", vp, vp, vp, u64, pu64)
     _sig(lib, "dampr_table_fetch", vp, vp, vp, vp, vp, u64, pu64)
@@ -452,11 +458,20 @@ class Table(object):
         s = FieldsSpec(int(sep), int(kf), int(kind), int(vf), int(op), 1 if cr_is_data else 0)
         self.ctx.check(self.ctx.lib.dampr_text_fields(self.ctx.h, self.h, tb.h, int(lo), int(hi), C.byref(s)))
 
+    def fields_records(self, tb, lo, hi, spec, kv, cr_is_data=False):
+        """Record mode of fields() (spec op OP_SUM_I64 or OP_SUM_F64): one {key code, value} record per line starting
+        in [lo, hi) into kv's buffer, in line order, holes {0, 0} for the lines left to the host; the table counts
+        the lines per key. fields_stats()["records"] is the scan's record count (kv's size is the caller's)."""
+        sep, kf, kind, vf, op = spec
+        s = FieldsSpec(int(sep), int(kf), int(kind), int(vf), int(op), 1 if cr_is_data else 0)
+        self.ctx.check(self.ctx.lib.dampr_text_fields_records(self.ctx.h, self.h, tb.h, int(lo), int(hi), C.byref(s),
+                                                              kv.h))
+
     def fields_stats(self):
         """stats() of a field scan under the names of its counters"""
         st = self.stats()
         return {"entries": st["entries"], "lines": st["lines"], "max_abs": st["empty"], "folded": st["folded"],
-                "flags": st["flags"], "hashed": st["hashed"], "fallback": st["fallback"]}
+                "flags": st["flags"], "hashed": st["hashed"], "fallback": st["fallback"], "records": st["raw"]}
 
     def fields_fetch(self, op):
         """(codes, values int64) of a field scan: the accumulators decoded from their MIN / MAX codes"""

@@ -292,6 +292,64 @@ def text_fields_spec(key_fn, value_fn, split_fn=None):
     return k[2], k[1], k[0], v[1]
 
 
+FIELD_FLOAT = "float"
+
+
+def _value_proj(e, record):
+    """(kind, j, sep) if e is int(record(e')[j]) (FIELD_INT) or float(record(e')[j]) (FIELD_FLOAT), else None"""
+    if isinstance(e, E) and e.op == "call" and isinstance(e.a, E) and e.a.op == "obj" and e.a.a is float \
+            and len(e.b) == 1:
+        p = _field_proj(e.b[0], record)
+        return None if p is None or p[0] != FIELD_STR else (FIELD_FLOAT, p[1], p[2])
+    p = _field_proj(e, record)
+    return p if p is not None and p[0] == FIELD_INT else None
+
+
+def _inline_call_of_arg(e):
+    """analyze(f) for e = f(x), x the argument and f a one-argument Python function (mean()'s `value(v)`): f's body
+    is then already an expression over x"""
+    if isinstance(e, E) and e.op == "call" and isinstance(e.a, E) and e.a.op == "obj" and len(e.b) == 1 \
+            and _is_arg(e.b[0]) and isinstance(e.a.a, types.FunctionType) and e.a.a.__code__.co_argcount == 1:
+        return analyze(e.a.a)
+    return None
+
+
+def text_fields_value_spec(key_fn, value_fn, split_fn=None):
+    """The shapes text_fields_spec leaves out that the record and float modes of the field scan take:
+    (sep, key_index, key_kind, value_index, value_kind, mean) where the key is as in text_fields_spec and either
+    the value is float(l.split(sep)[j]) (mean False), or it is mean()'s `(value(v), 1)` with value int() or float()
+    of l.split(sep)[j] (mean True). None for any other shape."""
+    fns = [f for f in (key_fn, value_fn, split_fn) if f is not None]
+    if not all(isinstance(f, types.FunctionType) and f.__code__.co_argcount == 1 for f in fns):
+        return None
+    ke, ve = analyze(key_fn), analyze(value_fn)
+    if ke is None or ve is None:
+        return None
+    if split_fn is None:
+        record = _split_sep
+    else:
+        sep = _split_sep(analyze(split_fn))
+        if sep is None:
+            return None
+
+        def record(x):
+            return sep if _is_arg(x) else None
+    k = _field_proj(ke, record)
+    if k is None:
+        return None
+    mean = False
+    if ve.op == "tuple" and len(ve.a) == 2:
+        ok, one = _const(ve.a[1])
+        inner = _inline_call_of_arg(ve.a[0])
+        if not ok or type(one) is not int or one != 1 or inner is None:
+            return None
+        ve, mean = inner, True
+    v = _value_proj(ve, record)
+    if v is None or v[2] != k[2] or (v[0] == FIELD_INT and not mean):
+        return None
+    return k[2], k[1], k[0], v[1], v[0], mean
+
+
 def field_index(fn):
     """i if fn is `lambda x: x[i]` with a constant non-negative int i, else None."""
     e = analyze(fn)

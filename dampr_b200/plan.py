@@ -466,14 +466,15 @@ class TextScan(object):
         self.host_lines = extra_lines
         return self
 
-    def _fetch_words(self, tab, tb, st, mode):
+    def _fetch_words(self, tab, tb, st, mode, want_codes=False):
         """(keys, counts) of the table: keys are materialised on the device (K9) as fixed-width ASCII; only tokens
-        longer than the width (rare) are patched on the host from their representative occurrence"""
+        longer than the width (rare) are patched on the host from their representative occurrence.
+        want_codes: (keys, counts, key codes)"""
         # exact codes hold at most 12 characters: without hashed tokens 16 bytes per key are enough and
         # neither codes nor representatives are needed on the host
         hashed = bool(st["hashed"])
         W = 32 if hashed else 16
-        words, counts, codes, reps = tab.fetch_words(tb, mode, W, with_codes=hashed)
+        words, counts, codes, reps = tab.fetch_words(tb, mode, W, with_codes=hashed or want_codes)
         too_long = np.flatnonzero(((codes >> np.uint64(63)) != 0) & ((reps & np.uint64(0xFFFFF)) > W)) if hashed else ()
         if len(too_long):
             wl = [b.decode("ascii") for b in words.tolist()]
@@ -482,7 +483,7 @@ class TextScan(object):
                 s = tb.download(rep >> 20, rep & 0xFFFFF).tobytes().decode("ascii")
                 wl[i] = s if mode == dev.TOK_WS else s.lower()
             words = wl
-        return words, counts
+        return (words, counts, codes) if want_codes else (words, counts)
 
     def _fallback_lines(self, tb, tab):
         """(offset, line) of every line on the table's fallback list, split by the reference's reader rules"""
@@ -690,42 +691,94 @@ class TextScan(object):
 
 class FieldScan(TextScan):
     """One pass of the delimited-field kernel (dampr_text_fields) over a text input: TextScan's ingest with the field
-    fold as the per-range launch. The lines the device hands back go through the stage's own functions."""
+    fold as the per-range launch. The lines the device hands back go through the stage's own functions.
+
+    Float sums and mean() run the kernel's record mode (dampr_text_fields_records): one {key code, value} record per
+    line in line order, folded by a stable device sort + segmented reduce, so a float sum is the same bits whatever
+    the chunking; the table counts the lines of each key (mean()'s count)."""
 
     HALO = dev.FIELDS_HALO   # a line longer than the kernel's window is measured up to 64 KB past its start
+    REC_BYTES = 32           # per record: the record and the sort's scratch copy
 
-    def __init__(self, runner, sources, spec, op, stage):
+    def __init__(self, runner, sources, spec, op, stage, mean=False):
         TextScan.__init__(self, runner, sources, None)
         self.spec = spec     # (separator byte, key index, key kind, value index or FIELD_VAL_ONE)
         self.op = op
         self.stage = stage
+        self.mean = mean     # values are mean()'s (sum, count) pairs
+        self.records = mean or op == dev.OP_SUM_F64
+        self.float_values = op in (dev.OP_SUM_F64, dev.OP_MIN_F64, dev.OP_MAX_F64)
         self.keys = self.values = None
         self.groups = self.host_lines = 0
+        self._rec = None     # record buffer (KV) and its capacity
+        self._rec_cap = 0
+        self._rec_regrown = False
 
     def _launch(self, tab, tb, lo, hi):
-        tab.fields(tb, lo, hi, tuple(self.spec) + (self.op,), getattr(self, "_cr_is_data", False))
+        spec = tuple(self.spec) + (self.op,)
+        if not self.records:
+            tab.fields(tb, lo, hi, spec, getattr(self, "_cr_is_data", False))
+            return
+        if self._rec is None:
+            # a first guess of one record per 32 bytes of text; a scan with more lines is repeated once with a
+            # buffer of the exact size (DAMPR_TF_RECFULL)
+            self._records_buffer(min(tb.n // 32 + 4096, self._free_bytes() // (2 * self.REC_BYTES)))
+        tab.fields_records(tb, lo, hi, spec, self._rec, getattr(self, "_cr_is_data", False))
+
+    def _free_bytes(self):
+        return int(self.runner.ctx.mem_info()[0])
+
+    def _records_buffer(self, n):
+        """a record buffer of n records, refused when it and the sort's scratch do not fit in device memory"""
+        held = self._rec_cap * 16
+        self._free_records()
+        if self.REC_BYTES * n > self._free_bytes() + held:
+            raise NotLowerable("field records and sort scratch (%d B per line) exceed free device memory"
+                               % self.REC_BYTES)
+        self._rec = self.runner.ctx.kv(max(1, n))
+        self._rec_cap = max(1, n)
+
+    def _free_records(self):
+        if self._rec is not None:
+            self._rec.free()
+        self._rec, self._rec_cap = None, 0
 
     def run(self):
+        try:
+            return self._run()
+        finally:
+            self._free_records()
+
+    def _run(self):
         _ctx, tb, tab, _st = self._ingest()
         st = tab.fields_stats()
         flags = st["flags"]
         if (flags & dev.TF_TABLEFULL or st["entries"] * 2 > tab.capacity) and settings.text_table_log2 < 28 \
                 and not resident_retry_block(self):
             settings.text_table_log2 = int(settings.text_table_log2) + 2   # as TextScan.run: a 4x table, scan again
-            return self.run()
+            return self._run()
         if flags & dev.TF_TABLEFULL:
             raise NotLowerable("combiner table overflow")
         if flags & (dev.TF_NONASCII | dev.TF_LONGLINE):
             raise NotLowerable("more lines for the host than the fallback list holds, or a line of 64 KB or more")
         if flags & dev.TF_COLLISION:
             raise NotLowerable("64-bit key-code collision between two long keys")
+        if self.float_values and flags & dev.TF_NEGZERO:
+            raise NotLowerable("-0.0 among the float() values: Python's result depends on the order of the arguments")
+        if self.records and flags & dev.TF_RECFULL:
+            if self._rec_regrown:
+                raise NotLowerable("field records overflow their buffer")
+            self._rec_regrown = True
+            self._records_buffer(int(st["records"]))   # the exact line count of the scan
+            return self._run()
         if self.spec[2] == dev.FIELD_KEY_INT:
             codes, acc, _reps = tab.fetch()
             keys = (codes ^ np.uint64(1 << 63)).view(np.int64)
+        elif self.records:
+            keys, acc, codes = self._fetch_words(tab, tb, st, dev.TOK_WS, want_codes=True)
         else:
             keys, acc = self._fetch_words(tab, tb, st, dev.TOK_WS)   # 7-bit codes: the str.split decoding
-        vals = dev.decode_fold(acc, self.op)
-        # the lines the device handed back: the stage's own mapper functions, folded with its binop
+        # the lines the device handed back: the stage's own mapper functions, folded with its binop in line order
         binop = self.stage.options.get("binop")
         extra, nrec, max_abs = {}, 0, 0
         if st["fallback"]:
@@ -734,16 +787,86 @@ class FieldScan(TextScan):
                 it = p.stream(it)
             for k, v in it:
                 nrec += 1
-                max_abs = max(max_abs, abs(v))
+                if not self.float_values:
+                    max_abs = max(max_abs, abs(v[0] if self.mean else v))
+                elif self.op != dev.OP_SUM_F64 and (v != v or (v == 0 and math.copysign(1.0, v) < 0)):
+                    raise NotLowerable("NaN or -0.0 under min/max")   # the result depends on the argument order
                 extra[k] = binop(extra[k], v) if k in extra else v
         # Python's ints are unbounded, the table's are 64-bit (SURVEY B12): the bound of _may_overflow
         if self.op == dev.OP_SUM_I64 and (int(st["folded"]) + nrec) * max(int(st["max_abs"]), max_abs) >= (1 << 62):
             raise NotLowerable("64-bit sum could overflow (SURVEY B12)")
-        self.keys, self.values = _merge_folds(keys, vals, extra, binop)
-        self.groups = len(self.values)
+        if not self.records:
+            vals = dev.decode_fold(acc, self.op)
+            if self.float_values:
+                self.keys, (self.values,) = _merge_fold_cols(keys, [vals], extra, binop)
+            else:
+                self.keys, self.values = _merge_folds(keys, vals, extra, binop)
+        else:
+            sums = self._record_sums(codes, int(st["records"]))
+            if self.mean:
+                self.keys, cols = _merge_fold_cols(keys, [sums, acc.view(np.int64)], extra, binop)
+                self.values = vexpr.Tup(cols)
+            else:
+                self.keys, (self.values,) = _merge_fold_cols(keys, [sums], extra, binop)
+        self.groups = len(self.keys)
         self.n_lines = int(st["lines"]) + nrec   # one record per line
         self.host_lines = nrec
         return self
+
+    def _record_sums(self, codes, n):
+        """per table key code (in `codes` order): the sum of its records' values, folded in line order by the stable
+        sort + segmented reduce (float64 under OP_SUM_F64, else int64)"""
+        # dampr_kv_sort_reduce allocates its scratch copy at the buffer's capacity and an output of n records
+        if 16 * (self._rec_cap + n) > self._free_bytes():
+            raise NotLowerable("the sort scratch of the field records exceeds free device memory")
+        kv, self._rec, self._rec_cap = self._rec, None, 0
+        try:
+            kv.set_size(n)
+            # KEY_MIX: packed str codes are far from uniform in their raw bits, and the sort's partitions follow the
+            # bits it sorts by. 2*10^7 records of 10^6 "u%07d" keys on an H100: leaf sort 153 ms under KEY_RAW,
+            # 1.6 ms under KEY_MIX. The stable sort keeps each key's records in line order either way.
+            red = kv.sort_reduce(self.op, dev.KEY_MIX)   # consumes kv
+        finally:
+            kv.free()
+        try:
+            rk, rv = red.columns()
+        finally:
+            red.free()
+        real = rk != 0                                  # the holes: key code 0
+        rk, rv = rk[real], rv[real]
+        order = np.argsort(rk)
+        rk, rv = rk[order], rv[order]
+        pos = np.searchsorted(rk, codes)
+        if len(codes) != len(rk) or (len(codes) and not np.array_equal(rk[np.minimum(pos, len(rk) - 1)], codes)):
+            raise NotLowerable("field records and table keys disagree")
+        return rv[pos].view(np.float64 if self.op == dev.OP_SUM_F64 else np.int64)
+
+
+def _key_positions(keys, extra):
+    """{key: index into keys} for the keys of `extra` that a device fold's `keys` ('S' array, int64 array or list of
+    str) holds"""
+    if isinstance(keys, np.ndarray) and keys.dtype.kind == "S":
+        W = keys.dtype.itemsize
+        fit = [k for k in extra if type(k) is str and k.isascii() and len(k) <= W and "\0" not in k]
+        probe = np.array([k.encode("ascii") for k in fit], dtype=keys.dtype)
+        hit = np.flatnonzero(np.isin(keys, probe)) if fit and len(keys) else np.zeros(0, dtype=np.int64)
+        return {b.decode("ascii"): i for b, i in zip(keys[hit].tolist(), hit.tolist())}
+    if isinstance(keys, np.ndarray):
+        fit = [k for k in extra if type(k) is int]
+        probe = np.array(fit, dtype=np.int64)
+        hit = np.flatnonzero(np.isin(keys, probe)) if fit and len(keys) else np.zeros(0, dtype=np.int64)
+        return dict(zip(keys[hit].tolist(), hit.tolist()))
+    return {k: i for i, k in enumerate(keys)}
+
+
+def _append_keys(keys, new):
+    """keys (as _key_positions) followed by the keys `new`, in the cheapest representation that holds them all"""
+    if isinstance(keys, np.ndarray) and keys.dtype.kind == "S" and \
+            all(type(k) is str and k.isascii() and len(k) <= keys.dtype.itemsize and "\0" not in k for k in new):
+        return np.concatenate((keys, np.array([k.encode("ascii") for k in new], dtype=keys.dtype)))
+    if isinstance(keys, np.ndarray) and keys.dtype.kind == "i" and all(type(k) is int for k in new):
+        return np.concatenate((keys, np.array(new, dtype=np.int64)))
+    return Frame._pylist(keys) + new
 
 
 def _merge_folds(keys, vals, extra, binop):
@@ -755,19 +878,7 @@ def _merge_folds(keys, vals, extra, binop):
             any(type(k) is int and not -(1 << 63) <= k < (1 << 63) for k in extra):
         raise NotLowerable("a host-folded value or key outside int64")
     vals = np.array(vals, dtype=np.int64, copy=True)
-    if isinstance(keys, np.ndarray) and keys.dtype.kind == "S":
-        W = keys.dtype.itemsize
-        fit = [k for k in extra if type(k) is str and k.isascii() and len(k) <= W and "\0" not in k]
-        probe = np.array([k.encode("ascii") for k in fit], dtype=keys.dtype)
-        hit = np.flatnonzero(np.isin(keys, probe)) if fit and len(keys) else np.zeros(0, dtype=np.int64)
-        pos = {b.decode("ascii"): i for b, i in zip(keys[hit].tolist(), hit.tolist())}
-    elif isinstance(keys, np.ndarray):
-        fit = [k for k in extra if type(k) is int]
-        probe = np.array(fit, dtype=np.int64)
-        hit = np.flatnonzero(np.isin(keys, probe)) if fit and len(keys) else np.zeros(0, dtype=np.int64)
-        pos = dict(zip(keys[hit].tolist(), hit.tolist()))
-    else:
-        pos = {k: i for i, k in enumerate(keys)}
+    pos = _key_positions(keys, extra)
     new = []
     for k, v in extra.items():
         i = pos.get(k) if type(k) in (str, int) else None
@@ -781,14 +892,45 @@ def _merge_folds(keys, vals, extra, binop):
     if not new:
         return keys, vals
     nv = np.array([extra[k] for k in new], dtype=np.int64)
-    if isinstance(keys, np.ndarray) and keys.dtype.kind == "S" and \
-            all(type(k) is str and k.isascii() and len(k) <= keys.dtype.itemsize and "\0" not in k for k in new):
-        keys = np.concatenate((keys, np.array([k.encode("ascii") for k in new], dtype=keys.dtype)))
-    elif isinstance(keys, np.ndarray) and keys.dtype.kind == "i" and all(type(k) is int for k in new):
-        keys = np.concatenate((keys, np.array(new, dtype=np.int64)))
-    else:
-        keys = Frame._pylist(keys) + new
-    return keys, np.concatenate((vals, nv))
+    return _append_keys(keys, new), np.concatenate((vals, nv))
+
+
+def _merge_fold_cols(keys, cols, extra, binop):
+    """_merge_folds for float64 values (one column) or mean()'s (sum, count) pairs (two columns, int64 or float64
+    sums): a key present in both gets binop(device value, host value); int64 columns must hold the results"""
+    if not extra:
+        return keys, cols
+    if any(type(k) is int and not -(1 << 63) <= k < (1 << 63) for k in extra):
+        raise NotLowerable("a host-folded key outside int64")
+    cols = [np.array(c, copy=True) for c in cols]
+
+    def parts(v):
+        return tuple(v) if len(cols) > 1 else (v,)
+
+    def fits(xs, c):
+        if c.dtype == np.float64:
+            return all(type(x) is float for x in xs)
+        return all(type(x) is int and -(1 << 63) <= x < (1 << 63) for x in xs)
+
+    pos = _key_positions(keys, extra)
+    new = []
+    for k, v in extra.items():
+        i = pos.get(k) if type(k) in (str, int) else None
+        if i is None:
+            new.append(k)
+            continue
+        dv = cols[0][i].item() if len(cols) == 1 else tuple(c[i].item() for c in cols)
+        r = parts(binop(dv, v))
+        if len(r) != len(cols) or not all(fits([x], c) for x, c in zip(r, cols)):
+            raise NotLowerable("a merged value the device columns do not hold")
+        for x, c in zip(r, cols):
+            c[i] = x
+    if not new:
+        return keys, cols
+    nv = [[parts(extra[k])[j] for k in new] for j in range(len(cols))]
+    if not all(len(parts(extra[k])) == len(cols) for k in new) or not all(fits(x, c) for x, c in zip(nv, cols)):
+        raise NotLowerable("a host-folded value the device columns do not hold")
+    return _append_keys(keys, new), [np.concatenate((c, np.array(x, dtype=c.dtype))) for c, x in zip(cols, nv)]
 
 
 def _source_key(sources):
@@ -873,6 +1015,41 @@ def _match_text_fields(stage, inputs):
                  dev.FIELD_VAL_ONE if vi is None else vi), _FOLD_OPS[kind]
 
 
+_FIELD_F64_OPS = {lowering.ADD: dev.OP_SUM_F64, lowering.MIN: dev.OP_MIN_F64, lowering.MAX: dev.OP_MAX_F64}
+_FIELD_OP_NAMES = {dev.OP_SUM_F64: "sum_f64", dev.OP_MIN_F64: "min_f64", dev.OP_MAX_F64: "max_f64"}
+
+
+def _match_text_fields_values(stage, inputs):
+    """[map(l.split(S)) ->] keyed(field key, float(field)) + PartialReduceCombiner(+ | min | max), or mean()'s
+    keyed(field key, (int(field) | float(field), 1)) + component-wise (+, +), over text:
+    (sources, (sep byte, key index, key kind, value index), op, mean) or None. Tried after _match_text_fields."""
+    if not isinstance(stage, GMap) or len(inputs) != 1:
+        return None
+    src = _text_files(inputs[0])
+    if src is None:
+        return None
+    ks = _opkinds(stage.mapper)
+    if ks is None or [k for k, _ in ks] not in (["keyed"], ["map", "keyed"]):
+        return None
+    if not isinstance(stage.combiner, ops.PartialReduceCombiner):
+        return None
+    keyed = ks[-1][1]
+    spec = lowering.text_fields_value_spec(keyed.fn, keyed.fn2, ks[0][1].fn if len(ks) == 2 else None)
+    if spec is None:
+        return None
+    sep, ki, kkind, vi, vkind, mean = spec
+    binop = stage.options.get("binop")
+    if mean:
+        if lowering.tuple_binop_kinds(binop) != [lowering.ADD, lowering.ADD]:
+            return None
+        op = dev.OP_SUM_F64 if vkind == lowering.FIELD_FLOAT else dev.OP_SUM_I64
+    else:
+        op = _FIELD_F64_OPS.get(lowering.binop_kind(binop))
+        if op is None:
+            return None
+    return src, (ord(sep), ki, dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR, vi), op, mean
+
+
 def _match_line_count(stage, inputs):
     if not isinstance(stage, GMap) or len(inputs) != 1:
         return None
@@ -948,6 +1125,17 @@ def _lower_map(runner, stage, inputs, si):
         runner.stats.add(stage, "device text fields scan+combine",
                          "bytes=%d lines=%d groups=%d host_lines=%d" % (scan.nbytes, scan.n_lines, scan.groups,
                                                                         scan.host_lines))
+        return Frame(scan.keys, [scan.values], scalar=True, combined=True)
+    m = _match_text_fields_values(stage, inputs)
+    if m is not None:
+        if dist.active():
+            raise NotLowerable("the field scan runs on one process")
+        src, spec, op, mean = m
+        scan = FieldScan(runner, src, spec, op, stage, mean=mean).run()
+        opname = ("mean_f64" if op == dev.OP_SUM_F64 else "mean_i64") if mean else _FIELD_OP_NAMES[op]
+        runner.stats.add(stage, "device text fields scan+combine",
+                         "op=%s bytes=%d lines=%d groups=%d host_lines=%d" % (opname, scan.nbytes, scan.n_lines,
+                                                                             scan.groups, scan.host_lines))
         return Frame(scan.keys, [scan.values], scalar=True, combined=True)
     if _match_line_count(stage, inputs):
         ds = inputs[0]

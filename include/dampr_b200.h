@@ -89,6 +89,7 @@ int32_t dampr_ctx_stream(dampr_ctx *ctx, uint64_t *out_stream);
 #define DAMPR_K_SYNTH 11
 #define DAMPR_K_MISC 12
 #define DAMPR_K_TEXT_FIELDS 13
+#define DAMPR_K_TEXT_FIELDS_COUNT 14   /* dampr_text_fields_records' line-count pass and tile scan */
 
 /* ---- pinned host memory (spill ring / ingest staging) -------------------------------- */
 int32_t dampr_host_alloc(uint64_t nbytes, void **out);
@@ -154,6 +155,8 @@ int32_t dampr_text_verify(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uin
 #define DAMPR_TF_TABLEFULL 8u
 #define DAMPR_TF_LONGTOKEN 16u
 #define DAMPR_TF_COLLISION 32u
+#define DAMPR_TF_RECFULL 64u   /* dampr_text_fields_records: more lines than the record buffer holds            */
+#define DAMPR_TF_NEGZERO 128u  /* a float() field scan parsed a negative zero                                    */
 int32_t dampr_table_stats(dampr_ctx *ctx, dampr_table *t, uint64_t stats[8]);
 /* Per-line fallback of the [^\w]+ tokenisers: a line that holds a byte the device cannot tokenise the way
  * Python does (non-ASCII: Unicode \w / lower(); '\r' in text mode: universal newlines) contributes NOTHING to
@@ -163,7 +166,7 @@ int32_t dampr_table_stats(dampr_ctx *ctx, dampr_table *t, uint64_t stats[8]);
  * returns *n only. More than 65536 such lines, or one that cannot be isolated inside the kernel's window, set
  * DAMPR_TF_NONASCII instead (the whole scan is then the caller's). str.split mode keeps scan-wide flags. */
 int32_t dampr_table_fallback_lines(dampr_ctx *ctx, dampr_table *t, uint64_t *lines, uint64_t cap, uint64_t *n);
-/* ---- delimited-field fold over text: replaces Map.stream of `l.split(S)[i]` keys with `1` / `int(l.split(S)[j])`
+/* ---- delimited-field fold over text: replaces Map.stream of `l.split(S)[i]` keys with `1` / `int()` / `float()` of `l.split(S)[j]`
  *      values (base.py:30-33) fused with ReducedWriter.add_record under +, min or max (dataset.py:100-105) -------- */
 #define DAMPR_FIELD_KEY_STR 0          /* key = line.split(sep)[key_field]                                   */
 #define DAMPR_FIELD_KEY_INT 1          /* key = int(line.split(sep)[key_field])                              */
@@ -175,26 +178,46 @@ typedef struct dampr_fields_spec {
     int32_t sep;        /* separator byte: ASCII, not NUL, '\n' or '\r'                                     */
     int32_t key_field;  /* i of line.split(sep)[i]; negative counts from the end, as in Python              */
     int32_t key_kind;   /* DAMPR_FIELD_KEY_STR | DAMPR_FIELD_KEY_INT                                         */
-    int32_t val_field;  /* j of int(line.split(sep)[j]), negative from the end, or DAMPR_FIELD_VAL_ONE          */
-    int32_t op;         /* DAMPR_OP_SUM_I64 | DAMPR_OP_MIN_I64 | DAMPR_OP_MAX_I64                            */
+    int32_t val_field;  /* j of int() / float() of line.split(sep)[j], negative from the end, or
+                           DAMPR_FIELD_VAL_ONE (int ops of dampr_text_fields only)                            */
+    int32_t op;         /* dampr_text_fields: DAMPR_OP_SUM_I64 | MIN_I64 | MAX_I64 (int() values) or
+                           DAMPR_OP_MIN_F64 | MAX_F64 (float() values); dampr_text_fields_records:
+                           DAMPR_OP_SUM_I64 (int() values) | DAMPR_OP_SUM_F64 (float() values)               */
     int32_t cr_is_data; /* 1: '\r' is an ordinary byte (binary-mode .gz); 0: it ends lines (text mode)        */
 } dampr_fields_spec;
 /* fold (key code -> value) of the lines whose first byte lies in [own_lo, own_hi) into the table (cleared by the
  * caller before the first range; ranges of one scan accumulate). Needs bytes [0, min(n, own_hi + DAMPR_FIELDS_HALO))
  * uploaded. The device folds a line only when every byte is ASCII and not NUL, it holds no '\r' (unless
- * cr_is_data), every field it reads exists, every int() field is exactly [+-]?[0-9]{1,18}, and it ends within
- * 4 KB of its start. Every other line goes onto the fallback list (dampr_table_fallback_lines) for the caller to
- * run its own functions on; more lines than the list holds set DAMPR_TF_NONASCII, a line of 64 KB or more sets
- * DAMPR_TF_LONGLINE (the whole scan is then the caller's).
+ * cr_is_data), every field it reads exists, every int() field is exactly [+-]?[0-9]{1,18}, every float() field is
+ * one the device parses to Python's bits ([ \t]*[+-]?(\d+\.?\d*|\.\d+)([eE][+-]?\d+)?[ \t]* with at most 19
+ * significant digits, see csrc/fparse.cuh), and it ends within 4 KB of its start. Every other line goes onto the
+ * fallback list (dampr_table_fallback_lines) for the caller to run its own functions on; more lines than the list
+ * holds set DAMPR_TF_NONASCII, a line of 64 KB or more sets DAMPR_TF_LONGLINE (the whole scan is then the caller's).
  * Key codes: str keys of 1..9 bytes pack 7 bits per byte (dampr_table_fetch_words with DAMPR_TOK_WS decodes them);
  * '' and longer keys are hashed codes (bit 63) with a representative occurrence, byte-compared on every insert
- * (DAMPR_TF_COLLISION on a mismatch); int keys v are v ^ 2^63.
+ * (DAMPR_TF_COLLISION on a mismatch); int keys v are v ^ 2^63. No key code is 0.
  * Accumulators (the table's counts): SUM = the two's-complement sum; MAX = v ^ 2^63 of the maximum; MIN =
- * ~(v ^ 2^63) of the minimum (order-preserving codes whose identity is the cleared 0).
+ * ~(v ^ 2^63) of the minimum (order-preserving codes whose identity is the cleared 0). MAX_F64 holds the code
+ * c = bits ^ (sign ? ~0 : 2^63) of the largest double, MIN_F64 ~c of the smallest. A parsed -0.0 sets
+ * DAMPR_TF_NEGZERO (Python's min / max of 0.0 and -0.0 depends on the order of the arguments).
  * dampr_table_stats after the scan: stats[0]=entries stats[1]=lines folded on the device stats[2]=max |value|
- * folded stats[3]=records folded (= stats[1]) stats[4]=flags stats[5]=hashed str keys stats[7]=fallback lines. */
+ * folded (int values) stats[3]=records folded (= stats[1]) stats[4]=flags stats[5]=hashed str keys
+ * stats[7]=fallback lines. */
 int32_t dampr_text_fields(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo, uint64_t own_hi,
                           const dampr_fields_spec *spec);
+/* record mode of the same scan, for folds whose result depends on the order of the values (float sums) or that
+ * need a count per key (mean()): one 16-byte record {key code, value} per line owned by [own_lo, own_hi) is written
+ * to rec's buffer, value = the int64 of int() (DAMPR_OP_SUM_I64) or the bits of float() (DAMPR_OP_SUM_F64). Records
+ * are in line order: the lines of one scan (the ranges since the table was cleared) take indices 0, 1, 2, ...
+ * whatever the ranges and the grid schedule. A line the device does not take (the fallback list, the rules above)
+ * is a hole record {0, 0}; key code 0 is never a real code. The table takes one insert per taken line and counts
+ * lines per key (its counts), keeps the representatives of hashed keys and checks them, exactly as above.
+ * stats[6] = records of the scan so far (taken lines + holes), the index the next range starts at. When the index
+ * reaches rec's capacity the kernel writes nothing past it and sets DAMPR_TF_RECFULL (stats[6] still counts every
+ * line: a buffer of that many records holds the scan). The caller sets rec's size (dampr_kv_set_size) from stats[6].
+ * Three kernels per range: a line count per 16 KB tile, one CTA's scan of the counts, the fold. */
+int32_t dampr_text_fields_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
+                                  uint64_t own_hi, const dampr_fields_spec *spec, dampr_kv *rec);
 /* compact the table into caller memory: codes[i], counts[i], reps[i] (rep = offset<<20 | len of the
  * lowest-offset occurrence, hashed tokens only, else 0). cap = array capacity; *n = entries written.
  * Pass all three arrays NULL to query *n only. Order is unspecified (dampr_table_to_kv +

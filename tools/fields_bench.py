@@ -6,6 +6,13 @@ from CUDA events (dampr_ctx_timings, DAMPR_K_TEXT_FIELDS) with its GB/s and shar
 page-cache-warm file, the host-map MB/s on a sample, and whether the device and the host results agree there.
 
     python tools/fields_bench.py [--gb 2] [--keys 1000000] [--reps 3] [--sample-mb 32] [--out DIR]
+                                 [--value int|float] [--op sum|min|max|mean]
+
+--value float writes the value field as float text (even lines "%.6f", odd lines repr() of the double, right-aligned
+in a 24-byte field) and folds float(r[2]); --op picks `+` (fold_by), min / max (a_group_by().reduce) or mean(). A run
+other than the default also reports every kernel's time by name (the record modes' count pass, fold and sort), and
+for float sums and means whether the sample agrees with Python within 4·n·2^-53·Σ|v| per key (plus one rounding for
+a mean); the default run prints exactly the fields it always printed.
 """
 import argparse
 import json
@@ -45,9 +52,83 @@ def csv_text(seed, n_lines, n_keys):
     return out.reshape(-1)
 
 
-def job(Dampr, src):
-    return Dampr.read_input(src).map(lambda l: l.split(",")) \
-        .fold_by(lambda r: r[0], value=lambda r: int(r[2]), binop=lambda a, b: a + b)
+FVAL = 24           # bytes of the float value field (--value float)
+
+
+def float_text(seed, n_lines, n_keys):
+    """the same layout with a 24-byte float value field: key, a 65-letter filler field, the value right-aligned in
+    spaces (Python's float() takes them), '\n'; even lines "%.6f", odd lines repr()"""
+    rng = np.random.default_rng(seed)
+    out = np.empty((n_lines, LINE), dtype=np.uint8)
+    keys = rng.integers(0, n_keys, size=n_lines)
+    out[:, 0] = ord("u")
+    for p in range(7):
+        out[:, 7 - p] = 48 + (keys // 10 ** p) % 10
+    out[:, 8] = ord(",")
+    vstart = LINE - 1 - FVAL
+    out[:, 9:vstart - 1] = rng.integers(97, 123, size=(n_lines, vstart - 10), dtype=np.uint8)
+    out[:, vstart - 1] = ord(",")
+    vals = rng.uniform(-1e5, 1e5, size=n_lines)
+    step = 1 << 20
+    for a in range(0, n_lines, step):
+        v = vals[a:a + step].tolist()
+        s = [("%.6f" % x if (a + i) % 2 == 0 else repr(x)).rjust(FVAL) for i, x in enumerate(v)]
+        out[a:a + len(s), vstart:LINE - 1] = np.frombuffer("".join(s).encode("ascii"), dtype=np.uint8).reshape(-1, FVAL)
+    out[:, LINE - 1] = ord("\n")
+    return out.reshape(-1)
+
+
+def job(Dampr, src, value="int", op="sum"):
+    conv = int if value == "int" else float
+    d = Dampr.read_input(src).map(lambda l: l.split(","))
+    if op == "mean":
+        return d.mean(lambda r: r[0], lambda r: conv(r[2]))
+    if op in ("min", "max"):
+        return d.a_group_by(lambda r: r[0], lambda r: conv(r[2])).reduce(min if op == "min" else max)
+    return d.fold_by(lambda r: r[0], value=lambda r: conv(r[2]), binop=lambda a, b: a + b)
+
+
+def python_fold(sample, value, op):
+    """the stage as plain Python over the sample's lines: {key: result}"""
+    conv = int if value == "int" else float
+    out = {}
+    for l in sample.decode("ascii").split("\n")[:-1]:
+        r = l.split(",")
+        k, v = r[0], conv(r[2])
+        if op == "mean":
+            s, n = out.get(k, (0, 0))
+            out[k] = (s + v, n + 1)
+        elif k in out:
+            out[k] = out[k] + v if op == "sum" else (min if op == "min" else max)(out[k], v)
+        else:
+            out[k] = v
+    if op == "mean":
+        out = {k: s / float(n) for k, (s, n) in out.items()}
+    return out
+
+
+def magnitudes(sample):
+    """{key: (lines, sum of |float value|)} of the sample: the scale of the sum bound"""
+    mag = {}
+    for l in sample.decode("ascii").split("\n")[:-1]:
+        r = l.split(",")
+        n, a = mag.get(r[0], (0, 0.0))
+        mag[r[0]] = (n + 1, a + abs(float(r[2])))
+    return mag
+
+
+def within_bound(got, host, mag, op):
+    """every key's device result within 4·n·2^-53·Σ|v| of Python's (plus one rounding of the result for a mean)"""
+    if set(got) != set(host):
+        return False
+    for k, hv in host.items():
+        n, a = mag[k]
+        tol = 4 * n * 2.0 ** -53 * a
+        if op == "mean":
+            tol = tol / n + abs(hv) * 2.0 ** -52
+        if abs(got[k] - hv) > 2 * tol:
+            return False
+    return True
 
 
 def card():
@@ -66,14 +147,17 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--sample-mb", type=float, default=32)
     ap.add_argument("--out", default=None, help="directory for the text file (default: a temporary one)")
+    ap.add_argument("--value", choices=("int", "float"), default="int")
+    ap.add_argument("--op", choices=("sum", "min", "max", "mean"), default="sum")
     a = ap.parse_args()
+    default = a.value == "int" and a.op == "sum"
 
     from dampr_b200 import Dampr, device as dev, plan
     from dampr_b200 import runner as runner_mod
     ctx = runner_mod.get_ctx()
     name, power = card()
     n_lines = int(a.gb * 1e9) // LINE
-    text = csv_text(2026, n_lines, a.keys)
+    text = csv_text(2026, n_lines, a.keys) if a.value == "int" else float_text(2026, n_lines, a.keys)
     nbytes = len(text)
     pin = dev.PinnedBuffer(nbytes)
     pin.array[:] = text
@@ -85,12 +169,16 @@ def main():
     def timed(src):
         ctx.timings_reset()
         t0 = time.perf_counter()
-        n = len(list(job(Dampr, src).run()))
+        n = len(list(job(Dampr, src, a.value, a.op).run()))
         dt = time.perf_counter() - t0
         stages = runner_mod.LAST_STATS.stages
         assert "device text fields scan+combine" in stages[0][1], stages
-        ms = sum(m for k, m in ctx.timings() if k == "text_fields")
-        return dt, ms, n, stages[0][2]
+        tm = ctx.timings()
+        ms = sum(m for k, m in tm if k == "text_fields")
+        by_name = {}
+        for k, m in tm:
+            by_name[k] = by_name.get(k, 0.0) + m
+        return dt, ms, n, stages[0][2], by_name
 
     ctx.timing_enable(True)
     timed(plan.MemoryText(pin.array))          # warm-up: module load, buffers, table size
@@ -106,15 +194,18 @@ def main():
     sample_lines = max(1, int(a.sample_mb * 1e6) // LINE)
     sample = pin.array[:sample_lines * LINE].tobytes()
     t0 = time.perf_counter()
-    host = {}
-    for l in sample.decode("ascii").split("\n")[:-1]:
-        r = l.split(",")
-        k, v = r[0], int(r[2])
-        host[k] = host[k] + v if k in host else v
+    if default:
+        host = {}
+        for l in sample.decode("ascii").split("\n")[:-1]:
+            r = l.split(",")
+            k, v = r[0], int(r[2])
+            host[k] = host[k] + v if k in host else v
+    else:
+        host = python_fold(sample, a.value, a.op)
     host_s = time.perf_counter() - t0
     spin = dev.PinnedBuffer(len(sample))
     spin.array[:] = np.frombuffer(sample, dtype=np.uint8)
-    got = dict(job(Dampr, plan.MemoryText(spin.array)).run())
+    got = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op).run())
 
     kernel_ms = min(m[1] for m in mem)
     res = {
@@ -134,6 +225,12 @@ def main():
         "sample_equal": got == host,
         "stats": mem[0][3],
     }
+    if not default:
+        best = min(mem, key=lambda m: m[0])
+        res.update({"value": a.value, "op": a.op,
+                    "kernels_ms": {k: round(v, 3) for k, v in sorted(best[4].items())}})
+        if a.value == "float" and a.op in ("sum", "mean"):
+            res["sample_within_bound"] = within_bound(got, host, magnitudes(sample), a.op)
     if a.out is None:
         shutil.rmtree(tmpdir, ignore_errors=True)
     print(json.dumps(res))
