@@ -228,7 +228,7 @@ def tokenizer_mode(fn):
     return None
 
 
-FIELD_STR, FIELD_INT = "str", "int"
+FIELD_STR, FIELD_INT, FIELD_FLOAT = "str", "int", "float"
 
 
 def _split_sep(e):
@@ -258,43 +258,6 @@ def _field_proj(e, record):
     return None if sep is None else (kind, i, sep)
 
 
-def text_fields_spec(key_fn, value_fn, split_fn=None):
-    """Device field-scan spec of a keyed(key_fn, value_fn) over text lines, optionally behind map(split_fn):
-    (sep, key_index, key_kind, value_index) where the key is l.split(sep)[key_index] (FIELD_STR) or its int()
-    (FIELD_INT), and the value is int(l.split(sep)[value_index]), or the constant 1 when value_index is None.
-    Indices may be negative (Python's from-the-end). None for any other shape."""
-    fns = [f for f in (key_fn, value_fn, split_fn) if f is not None]
-    if not all(isinstance(f, types.FunctionType) and f.__code__.co_argcount == 1 for f in fns):
-        return None
-    ke, ve = analyze(key_fn), analyze(value_fn)
-    if ke is None or ve is None:
-        return None
-    if split_fn is None:
-        record = _split_sep                      # the split is inside the key / value functions
-    else:
-        sep = _split_sep(analyze(split_fn))
-        if sep is None:
-            return None
-
-        def record(x):                           # key / value functions index the split record
-            return sep if _is_arg(x) else None
-    k = _field_proj(ke, record)
-    if k is None:
-        return None
-    ok, one = _const(ve)
-    if ok:
-        if type(one) is not int or one != 1:
-            return None
-        return k[2], k[1], k[0], None
-    v = _field_proj(ve, record)
-    if v is None or v[0] != FIELD_INT or v[2] != k[2]:
-        return None
-    return k[2], k[1], k[0], v[1]
-
-
-FIELD_FLOAT = "float"
-
-
 def _value_proj(e, record):
     """(kind, j, sep) if e is int(record(e')[j]) (FIELD_INT) or float(record(e')[j]) (FIELD_FLOAT), else None"""
     if isinstance(e, E) and e.op == "call" and isinstance(e.a, E) and e.a.op == "obj" and e.a.a is float \
@@ -314,11 +277,19 @@ def _inline_call_of_arg(e):
     return None
 
 
-def text_fields_value_spec(key_fn, value_fn, split_fn=None):
-    """The shapes text_fields_spec leaves out that the record and float modes of the field scan take:
-    (sep, key_index, key_kind, value_index, value_kind, mean) where the key is as in text_fields_spec and either
-    the value is float(l.split(sep)[j]) (mean False), or it is mean()'s `(value(v), 1)` with value int() or float()
-    of l.split(sep)[j] (mean True). None for any other shape."""
+def _is_one(e):
+    ok, v = _const(e)
+    return ok and type(v) is int and v == 1
+
+
+def text_fields_spec(key_fn, value_fn, split_fn=None):
+    """Device field-scan spec of a keyed(key_fn, value_fn) over text lines, optionally behind map(split_fn):
+    (sep, key_index, key_kind, value_index, value_kind, mean) where the key is l.split(sep)[key_index] (FIELD_STR) or
+    its int() (FIELD_INT), and the value is
+      the constant 1                                   value_index None, FIELD_INT, mean False
+      int() or float() of l.split(sep)[value_index]    FIELD_INT or FIELD_FLOAT, mean False
+      mean()'s `(value(v), 1)`, value one of those     FIELD_INT or FIELD_FLOAT, mean True
+    Indices may be negative (Python's from-the-end). None for any other shape."""
     fns = [f for f in (key_fn, value_fn, split_fn) if f is not None]
     if not all(isinstance(f, types.FunctionType) and f.__code__.co_argcount == 1 for f in fns):
         return None
@@ -326,26 +297,27 @@ def text_fields_value_spec(key_fn, value_fn, split_fn=None):
     if ke is None or ve is None:
         return None
     if split_fn is None:
-        record = _split_sep
+        record = _split_sep                      # the split is inside the key / value functions
     else:
         sep = _split_sep(analyze(split_fn))
         if sep is None:
             return None
 
-        def record(x):
+        def record(x):                           # key / value functions index the split record
             return sep if _is_arg(x) else None
     k = _field_proj(ke, record)
     if k is None:
         return None
-    mean = False
-    if ve.op == "tuple" and len(ve.a) == 2:
-        ok, one = _const(ve.a[1])
+    if _is_one(ve):
+        return k[2], k[1], k[0], None, FIELD_INT, False
+    mean = ve.op == "tuple" and len(ve.a) == 2
+    if mean:
         inner = _inline_call_of_arg(ve.a[0])
-        if not ok or type(one) is not int or one != 1 or inner is None:
+        if inner is None or not _is_one(ve.a[1]):
             return None
-        ve, mean = inner, True
+        ve = inner
     v = _value_proj(ve, record)
-    if v is None or v[2] != k[2] or (v[0] == FIELD_INT and not mean):
+    if v is None or v[2] != k[2]:
         return None
     return k[2], k[1], k[0], v[1], v[0], mean
 

@@ -409,16 +409,22 @@ class TextScan(object):
             st = dict(st, flags=st["flags"] & ~dev.TF_CR)
         return ctx, tb, tab, st
 
+    def _grow_table(self, tab, st):
+        """True when the table was made 4x larger for a repeated scan: it is full or over half full, below 2^28
+        entries, and the scan has retries left. ReducedWriter would flush a run here (dataset.py:107-113); with HBM
+        to spare the table is simply made larger (later scans start at the new size)."""
+        if (st["flags"] & dev.TF_TABLEFULL or st["entries"] * 2 > tab.capacity) and settings.text_table_log2 < 28 \
+                and not resident_retry_block(self):
+            settings.text_table_log2 = int(settings.text_table_log2) + 2
+            return True
+        return False
+
     def run(self):
         ctx, tb, tab, st = self._ingest()
         flags = st["flags"]
         if dist.active():
             return self._finish_distributed(ctx, tb, tab, st)
-        if (flags & dev.TF_TABLEFULL or st["entries"] * 2 > tab.capacity) and settings.text_table_log2 < 28 \
-                and not resident_retry_block(self):
-            # ReducedWriter would flush a run here (dataset.py:107-113); with HBM to spare the table
-            # is simply made 4x larger and the scan repeated (later scans start at the new size)
-            settings.text_table_log2 = int(settings.text_table_log2) + 2
+        if self._grow_table(tab, st):
             return self.run()
         if flags & dev.TF_TABLEFULL:
             raise NotLowerable("combiner table overflow")
@@ -700,7 +706,7 @@ class FieldScan(TextScan):
     HALO = dev.FIELDS_HALO   # a line longer than the kernel's window is measured up to 64 KB past its start
     REC_BYTES = 32           # per record: the record and the sort's scratch copy
 
-    def __init__(self, runner, sources, spec, op, stage, mean=False):
+    def __init__(self, runner, sources, spec, op, stage, mean):
         TextScan.__init__(self, runner, sources, None)
         self.spec = spec     # (separator byte, key index, key kind, value index or FIELD_VAL_ONE)
         self.op = op
@@ -753,9 +759,7 @@ class FieldScan(TextScan):
         _ctx, tb, tab, _st = self._ingest()
         st = tab.fields_stats()
         flags = st["flags"]
-        if (flags & dev.TF_TABLEFULL or st["entries"] * 2 > tab.capacity) and settings.text_table_log2 < 28 \
-                and not resident_retry_block(self):
-            settings.text_table_log2 = int(settings.text_table_log2) + 2   # as TextScan.run: a 4x table, scan again
+        if self._grow_table(tab, st):
             return self._run()
         if flags & dev.TF_TABLEFULL:
             raise NotLowerable("combiner table overflow")
@@ -796,11 +800,7 @@ class FieldScan(TextScan):
         if self.op == dev.OP_SUM_I64 and (int(st["folded"]) + nrec) * max(int(st["max_abs"]), max_abs) >= (1 << 62):
             raise NotLowerable("64-bit sum could overflow (SURVEY B12)")
         if not self.records:
-            vals = dev.decode_fold(acc, self.op)
-            if self.float_values:
-                self.keys, (self.values,) = _merge_fold_cols(keys, [vals], extra, binop)
-            else:
-                self.keys, self.values = _merge_folds(keys, vals, extra, binop)
+            self.keys, (self.values,) = _merge_fold_cols(keys, [dev.decode_fold(acc, self.op)], extra, binop)
         else:
             sums = self._record_sums(codes, int(st["records"]))
             if self.mean:
@@ -869,35 +869,11 @@ def _append_keys(keys, new):
     return Frame._pylist(keys) + new
 
 
-def _merge_folds(keys, vals, extra, binop):
-    """(keys, int64 values) of a device fold plus {key: value} folded on the host: a key present in both gets
-    binop(device value, host value). `keys` is an 'S' array, an int64 array or a list of str."""
-    if not extra:
-        return keys, vals
-    if any(not -(1 << 63) <= v < (1 << 63) for v in extra.values()) or \
-            any(type(k) is int and not -(1 << 63) <= k < (1 << 63) for k in extra):
-        raise NotLowerable("a host-folded value or key outside int64")
-    vals = np.array(vals, dtype=np.int64, copy=True)
-    pos = _key_positions(keys, extra)
-    new = []
-    for k, v in extra.items():
-        i = pos.get(k) if type(k) in (str, int) else None
-        if i is None:
-            new.append(k)
-            continue
-        r = binop(int(vals[i]), v)
-        if not -(1 << 63) <= r < (1 << 63):
-            raise NotLowerable("a merged value outside int64")
-        vals[i] = r
-    if not new:
-        return keys, vals
-    nv = np.array([extra[k] for k in new], dtype=np.int64)
-    return _append_keys(keys, new), np.concatenate((vals, nv))
-
-
 def _merge_fold_cols(keys, cols, extra, binop):
-    """_merge_folds for float64 values (one column) or mean()'s (sum, count) pairs (two columns, int64 or float64
-    sums): a key present in both gets binop(device value, host value); int64 columns must hold the results"""
+    """(keys, value columns) of a device fold plus {key: value} folded on the host: a key present in both gets
+    binop(device value, host value). The columns are one int64 or float64 column, or mean()'s (sum, count) pairs
+    (int64 or float64 sums, int64 counts); `keys` is an 'S' array, an int64 array or a list of str. An int64 column
+    must hold every host-folded value as well as every merged one."""
     if not extra:
         return keys, cols
     if any(type(k) is int and not -(1 << 63) <= k < (1 << 63) for k in extra):
@@ -912,6 +888,10 @@ def _merge_fold_cols(keys, cols, extra, binop):
             return all(type(x) is float for x in xs)
         return all(type(x) is int and -(1 << 63) <= x < (1 << 63) for x in xs)
 
+    # checked before the merge: a 20-digit host value under min or max sends the stage to the host even when the
+    # device value of its key is the one the merge keeps
+    if not all(fits([x], c) for v in extra.values() for x, c in zip(parts(v), cols) if c.dtype == np.int64):
+        raise NotLowerable("a host-folded value outside int64")
     pos = _key_positions(keys, extra)
     new = []
     for k, v in extra.items():
@@ -991,8 +971,9 @@ def _match_text_count(stage, inputs):
 
 
 def _match_text_fields(stage, inputs):
-    """[map(l.split(S)) ->] keyed(field key, 1 | int(field)) + PartialReduceCombiner(+ | min | max) over text:
-    (sources, (sep byte, key index, key kind, value index or FIELD_VAL_ONE), op) or None"""
+    """[map(l.split(S)) ->] keyed(field key, 1 | int(field) | float(field)) + PartialReduceCombiner(+ | min | max),
+    or mean()'s keyed(field key, (int(field) | float(field), 1)) + component-wise (+, +), over text:
+    (sources, (sep byte, key index, key kind, value index or FIELD_VAL_ONE), op, mean) or None"""
     if not isinstance(stage, GMap) or len(inputs) != 1:
         return None
     src = _text_files(inputs[0])
@@ -1002,39 +983,9 @@ def _match_text_fields(stage, inputs):
     if ks is None or [k for k, _ in ks] not in (["keyed"], ["map", "keyed"]):
         return None
     if not isinstance(stage.combiner, ops.PartialReduceCombiner):
-        return None
-    kind = lowering.binop_kind(stage.options.get("binop"))
-    if kind not in (lowering.ADD, lowering.MIN, lowering.MAX):
         return None
     keyed = ks[-1][1]
     spec = lowering.text_fields_spec(keyed.fn, keyed.fn2, ks[0][1].fn if len(ks) == 2 else None)
-    if spec is None:
-        return None
-    sep, ki, kkind, vi = spec
-    return src, (ord(sep), ki, dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR,
-                 dev.FIELD_VAL_ONE if vi is None else vi), _FOLD_OPS[kind]
-
-
-_FIELD_F64_OPS = {lowering.ADD: dev.OP_SUM_F64, lowering.MIN: dev.OP_MIN_F64, lowering.MAX: dev.OP_MAX_F64}
-_FIELD_OP_NAMES = {dev.OP_SUM_F64: "sum_f64", dev.OP_MIN_F64: "min_f64", dev.OP_MAX_F64: "max_f64"}
-
-
-def _match_text_fields_values(stage, inputs):
-    """[map(l.split(S)) ->] keyed(field key, float(field)) + PartialReduceCombiner(+ | min | max), or mean()'s
-    keyed(field key, (int(field) | float(field), 1)) + component-wise (+, +), over text:
-    (sources, (sep byte, key index, key kind, value index), op, mean) or None. Tried after _match_text_fields."""
-    if not isinstance(stage, GMap) or len(inputs) != 1:
-        return None
-    src = _text_files(inputs[0])
-    if src is None:
-        return None
-    ks = _opkinds(stage.mapper)
-    if ks is None or [k for k, _ in ks] not in (["keyed"], ["map", "keyed"]):
-        return None
-    if not isinstance(stage.combiner, ops.PartialReduceCombiner):
-        return None
-    keyed = ks[-1][1]
-    spec = lowering.text_fields_value_spec(keyed.fn, keyed.fn2, ks[0][1].fn if len(ks) == 2 else None)
     if spec is None:
         return None
     sep, ki, kkind, vi, vkind, mean = spec
@@ -1044,10 +995,16 @@ def _match_text_fields_values(stage, inputs):
             return None
         op = dev.OP_SUM_F64 if vkind == lowering.FIELD_FLOAT else dev.OP_SUM_I64
     else:
-        op = _FIELD_F64_OPS.get(lowering.binop_kind(binop))
-        if op is None:
+        kind = lowering.binop_kind(binop)
+        if kind not in (lowering.ADD, lowering.MIN, lowering.MAX):
             return None
-    return src, (ord(sep), ki, dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR, vi), op, mean
+        op = (_FOLD_OPS_F64 if vkind == lowering.FIELD_FLOAT else _FOLD_OPS)[kind]
+    return src, (ord(sep), ki, dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR,
+                 dev.FIELD_VAL_ONE if vi is None else vi), op, mean
+
+
+_FIELD_OP_NAMES = {dev.OP_SUM_I64: "sum_i64", dev.OP_MIN_I64: "min_i64", dev.OP_MAX_I64: "max_i64",
+                   dev.OP_SUM_F64: "sum_f64", dev.OP_MIN_F64: "min_f64", dev.OP_MAX_F64: "max_f64"}
 
 
 def _match_line_count(stage, inputs):
@@ -1120,19 +1077,10 @@ def _lower_map(runner, stage, inputs, si):
     if m is not None:
         if dist.active():
             raise NotLowerable("the field scan runs on one process")
-        src, spec, op = m
-        scan = FieldScan(runner, src, spec, op, stage).run()
-        runner.stats.add(stage, "device text fields scan+combine",
-                         "bytes=%d lines=%d groups=%d host_lines=%d" % (scan.nbytes, scan.n_lines, scan.groups,
-                                                                        scan.host_lines))
-        return Frame(scan.keys, [scan.values], scalar=True, combined=True)
-    m = _match_text_fields_values(stage, inputs)
-    if m is not None:
-        if dist.active():
-            raise NotLowerable("the field scan runs on one process")
         src, spec, op, mean = m
-        scan = FieldScan(runner, src, spec, op, stage, mean=mean).run()
-        opname = ("mean_f64" if op == dev.OP_SUM_F64 else "mean_i64") if mean else _FIELD_OP_NAMES[op]
+        scan = FieldScan(runner, src, spec, op, stage, mean).run()
+        opname = ("mean_f64" if op == dev.OP_SUM_F64 else "mean_i64") if mean else \
+            "count" if spec[3] == dev.FIELD_VAL_ONE and op == dev.OP_SUM_I64 else _FIELD_OP_NAMES[op]
         runner.stats.add(stage, "device text fields scan+combine",
                          "op=%s bytes=%d lines=%d groups=%d host_lines=%d" % (opname, scan.nbytes, scan.n_lines,
                                                                              scan.groups, scan.host_lines))

@@ -8,7 +8,8 @@ import os
 import numpy as np
 import pytest
 
-from test_text_fields_lowering import NEEDLE, PIPELINES, datasets, python_fold, reference_outputs, write_files
+from fields_standin import python_fold, reference_outputs, write_files
+from test_text_fields_lowering import GOLDEN, NEEDLE, PIPELINES, datasets
 
 pytestmark = pytest.mark.gpu
 
@@ -38,7 +39,7 @@ SUM = "Dampr.text(P).a_group_by(lambda l: l.split('%s')[%d], lambda l: int(l.spl
 def test_reference_inputs(name, engine, tmp_path):
     files = datasets()[name]
     P = write_files(tmp_path, files)
-    for src, exp in zip(PIPELINES[name], reference_outputs(files, PIPELINES[name])):
+    for src, exp in zip(PIPELINES[name], reference_outputs(files, PIPELINES[name], GOLDEN)):
         got, (_s, how, _d) = run(src, P)
         assert got == exp, (name, src)
         assert NEEDLE in how, (name, src, how)

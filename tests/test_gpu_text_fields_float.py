@@ -11,9 +11,9 @@ import zlib
 import numpy as np
 import pytest
 
+from fields_standin import python_lines, reference_outputs, write_files
 from test_fparse_host import corpus, in_grammar
-from test_text_fields_float_lowering import (NEEDLE, PIPELINES, datasets, python_lines, reference_outputs,
-                                             same_records, write_files, _kv_fns)
+from test_text_fields_float_lowering import GOLDEN, NEEDLE, PIPELINES, datasets, same_records, _kv_fns
 
 pytestmark = pytest.mark.gpu
 
@@ -43,7 +43,7 @@ def bits(v):
 def test_reference_inputs(name, engine, tmp_path):
     files = datasets()[name]
     P = write_files(tmp_path, files)
-    for src, exp in zip(PIPELINES[name], reference_outputs(files, PIPELINES[name])):
+    for src, exp in zip(PIPELINES[name], reference_outputs(files, PIPELINES[name], GOLDEN)):
         got, (_s, how, _d) = run(src, P)
         k, v, _m = _kv_fns(src)
         same_records(got, exp, P, k, v)

@@ -9,7 +9,7 @@ import pytest
 
 import text_contract as tc
 from oracle import refsem
-from test_text_fields_lowering import python_fold
+from fields_standin import python_fold
 
 MODES = (tc.TOK_WS, tc.TOK_NONWORD_LOWER_SET, tc.TOK_NONWORD_LOWER)
 

@@ -1,69 +1,22 @@
 """Float columns of delimited text: `float(l.split(S)[j])` sums, minima and maxima and `mean()` of int() or float()
-fields. The matcher (lowering.text_fields_value_spec), the planner's three modes (plan.FieldScan with MIN_F64 /
-MAX_F64 table codes, float sums and mean() through record mode) on a numpy stand-in for dampr_text_fields and
-dampr_text_fields_records defined here, and the results against the REAL reference (Refefer/Dampr), whose outputs
-are stored in tests/golden/text_fields_float.json.gz (DAMPR_REFERENCE=<checkout> records them again). Counts,
-minima and maxima are compared exactly, sums and means within 4·n·2^-53·Σ|v| (DESIGN §9). The same pipelines run on
-the device in tests/test_gpu_text_fields_float.py."""
+fields. The matcher (lowering.text_fields_spec), the planner's three modes (plan.FieldScan with MIN_F64 / MAX_F64
+table codes, float sums and mean() through record mode) on the numpy stand-in for dampr_text_fields and
+dampr_text_fields_records in tests/fields_standin.py, and the results against the REAL reference (Refefer/Dampr),
+whose outputs are stored in tests/golden/text_fields_float.json.gz (DAMPR_REFERENCE=<checkout> records them again).
+Counts, minima and maxima are compared exactly, sums and means within 4·n·2^-53·Σ|v| (DESIGN §9). The same pipelines
+run on the device in tests/test_gpu_text_fields_float.py."""
 import ast
-import gzip
-import hashlib
-import json
 import math
 import os
 import random
 import re
-import struct
-import subprocess as _subprocess
-import sys
 
-import numpy as np
 import pytest
 
-REF = os.environ.get("DAMPR_REFERENCE", "")
+from fields_standin import make_ctx, python_lines, reference_outputs, run_ours, write_files
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "text_fields_float.json.gz")
 NEEDLE = "device text fields scan+combine"
-
-DRIVER = r"""
-import sys, json, os, gzip, tempfile
-sys.path.insert(0, sys.argv[1])
-from dampr import Dampr
-d = tempfile.mkdtemp()
-for name, text in json.loads(sys.argv[2]):
-    with (gzip.open if name.endswith(".gz") else open)(os.path.join(d, name), "wb") as f:
-        f.write(text.encode("utf-8"))
-P = d if len(json.loads(sys.argv[2])) > 1 else os.path.join(d, json.loads(sys.argv[2])[0][0])
-print(json.dumps([sorted(repr(x) for x in eval(src).run()) for src in json.loads(sys.argv[3])]))
-"""
-
-
-def reference_outputs(files, srcs):
-    """the reference's output records (sorted reprs) of every pipeline in srcs over the files ([name, text])"""
-    args = [DRIVER, json.dumps(files), json.dumps(srcs)]
-    key = hashlib.sha256("\0".join(args).encode()).hexdigest()[:20]
-    runs = {}
-    if os.path.exists(GOLDEN):
-        with gzip.open(GOLDEN, "rb") as f:
-            runs = json.loads(f.read())
-    if REF:
-        env = dict(os.environ)
-        env.pop("PYTHONPATH", None)
-        p = _subprocess.run([sys.executable, "-c", DRIVER, REF] + args[1:], capture_output=True, text=True, env=env,
-                            cwd="/tmp", timeout=600)
-        assert p.returncode == 0, p.stderr[-2000:]
-        runs[key] = p.stdout.strip().split("\n")[-1]
-        with gzip.GzipFile(GOLDEN, "wb", mtime=0) as f:
-            f.write(json.dumps(runs, sort_keys=True).encode())
-    assert key in runs, "no recorded reference output for these inputs: record with DAMPR_REFERENCE=<checkout>"
-    return json.loads(runs[key])
-
-
-def write_files(d, files):
-    for name, text in files:
-        with (gzip.open if name.endswith(".gz") else open)(os.path.join(str(d), name), "wb") as f:
-            f.write(text.encode("utf-8"))
-    return str(d) if len(files) > 1 else os.path.join(str(d), files[0][0])
-
 
 # ---- inputs -----------------------------------------------------------------------------------------------------
 FLOAT_POOL = ["1.5", "-2.25", "0.1", "3", "1e3", "2.5E-3", ".5", "7.", "+4.75", " 8.125", "9.5 ", "1_0.5", "12.0",
@@ -112,201 +65,7 @@ PIPELINES = {
 PIPELINES["gz"] = PIPELINES["tsv"]
 
 
-# ---- numpy stand-in for dampr_text_fields (float ops) and dampr_text_fields_records ------------------------------
-GRAMMAR = re.compile(rb"[ \t]*[+-]?([0-9]+\.?[0-9]*|\.[0-9]+)([eE][+-]?[0-9]+)?[ \t]*\Z")
-
-
-def parse_f64(b):
-    """the header's float() rule: Python's value of the strings the device takes, else None"""
-    m = GRAMMAR.match(b)
-    if not m or len(m.group(1).replace(b".", b"").lstrip(b"0")) > 19:
-        return None
-    return float(b)
-
-
-def _int18(b):
-    s = b[1:] if b[:1] in (b"+", b"-") else b
-    if not (1 <= len(s) <= 18 and s.isdigit()):
-        return None
-    return -int(s) if b[:1] == b"-" else int(s)
-
-
-def f64_bits(v):
-    return struct.unpack("<Q", struct.pack("<d", v))[0]
-
-
-M64 = (1 << 64) - 1
-
-
-def make_ctx(free_bytes=1 << 30):
-    from fake_device import FakeTextCtx, FakeTable, FakeKV
-    from dampr_b200 import device as dev
-
-    class RecKV(FakeKV):
-        """a kv whose buffers count against the context's free memory, as device allocations do"""
-        def __init__(self, ctx, capacity):
-            FakeKV.__init__(self, ctx, capacity)
-            ctx.live[id(self)] = 16 * capacity
-
-        def set_size(self, n):
-            assert n <= len(self.rec)
-            self.n = int(n)
-
-        def sort_reduce(self, op, xform, sorted_run=False):
-            # dampr_kv_sort_reduce: a scratch copy at the capacity and an output of n records, or DAMPR_ERR_NOMEM
-            if 16 * (len(self.rec) + self.n) > self.ctx.mem_info()[0]:
-                raise dev.DeviceError("libdampr_b200 status -3: out of device memory")
-            return FakeKV.sort_reduce(self, op, xform, sorted_run)
-
-        def free(self):
-            self.ctx.live.pop(id(self), None)
-
-    class FieldsTable(FakeTable):
-        def clear(self):
-            FakeTable.clear(self)
-            self.acc, self.rep, self.code, self.max_abs = {}, {}, {}, 0
-
-        def _scan(self, tb, lo, hi, spec, cr_is_data, rec):
-            sep, kf, kind, vf, op = spec
-            data = tb.buf[:tb.n].tobytes()
-            pos = 0
-            while pos < len(data):
-                end = data.find(b"\n", pos)
-                end = len(data) if end < 0 else end
-                if lo <= pos < hi:
-                    self._line(data[pos:end], pos, bytes([sep]), kf, kind, vf, op, cr_is_data, rec)
-                pos = end + 1
-
-        def fields(self, tb, lo, hi, spec, cr_is_data=False):
-            assert spec[4] in (dev.OP_MIN_F64, dev.OP_MAX_F64)
-            self._scan(tb, lo, hi, spec, cr_is_data, None)
-
-        def fields_records(self, tb, lo, hi, spec, kv, cr_is_data=False):
-            assert spec[4] in (dev.OP_SUM_I64, dev.OP_SUM_F64)
-            self._scan(tb, lo, hi, spec, cr_is_data, kv)
-
-        def _line(self, line, off, sep, kf, kind, vf, op, cr_is_data, rec):
-            st = self.st
-            f = line.split(sep)
-            ok = len(line) < 4096 and all(0 < c < 0x80 for c in line) and (cr_is_data or b"\r" not in line)
-            ok = ok and -len(f) <= kf < len(f) and -len(f) <= vf < len(f)
-            flt = op != dev.OP_SUM_I64
-            v = (parse_f64(f[vf]) if flt else _int18(f[vf])) if ok else None
-            k = f[kf] if ok else None
-            if ok and kind == dev.FIELD_KEY_INT:
-                k = _int18(k)
-            if not ok or v is None or k is None:
-                if len(line) > 0xFFFF:
-                    st["flags"] |= dev.TF_LONGLINE
-                elif len(self.fb) < (1 << 16):
-                    self.fb.append((off << 16) | len(line))
-                    st["fallback"] += 1
-                else:
-                    st["flags"] |= dev.TF_NONASCII
-                if rec is not None:
-                    self._put(rec, 0, 0)
-                return
-            st["lines"] += 1
-            st["folded"] += 1
-            if flt and v == 0 and math.copysign(1.0, v) < 0:
-                st["flags"] |= dev.TF_NEGZERO
-            if not flt:
-                self.max_abs = max(self.max_abs, abs(v))
-            if kind == dev.FIELD_KEY_STR and not 1 <= len(k) <= 9:
-                st["hashed"] += 1
-                off_k = off + sum(len(x) + 1 for x in f[:kf if kf >= 0 else len(f) + kf])
-                self.rep[k] = min(self.rep.get(k, 1 << 62), (off_k << 20) | len(k))
-            if k not in self.code:
-                i = len(self.code)
-                self.code[k] = ((k ^ (1 << 63)) & M64 if kind == dev.FIELD_KEY_INT else
-                                (1 << 63 | i) if kind == dev.FIELD_KEY_STR and not 1 <= len(k) <= 9 else i + 1)
-            if rec is not None:
-                self._put(rec, self.code[k], f64_bits(v) if flt else v & M64)
-                self.acc[k] = self.acc.get(k, 0) + 1
-                return
-            b = f64_bits(v)
-            enc = b ^ (M64 if b >> 63 else 1 << 63)
-            if op == dev.OP_MIN_F64:
-                enc = ~enc & M64
-            self.acc[k] = max(self.acc.get(k, 0), enc)
-
-        def _put(self, kv, code, bits):
-            i = self.st["raw"]
-            self.st["raw"] += 1
-            if i < len(kv.rec):
-                kv.rec[i] = (code, bits)
-            else:
-                self.st["flags"] |= dev.TF_RECFULL
-
-        def stats(self):
-            d = dict(self.st, entries=len(self.acc), empty=self.max_abs)
-            if len(self.acc) * 2 > self.capacity and len(self.acc) >= self.capacity:
-                d["flags"] |= dev.TF_TABLEFULL
-            return d
-
-        def fields_stats(self):
-            st = self.stats()
-            return {"entries": st["entries"], "lines": st["lines"], "max_abs": st["empty"], "folded": st["folded"],
-                    "flags": st["flags"], "hashed": st["hashed"], "fallback": st["fallback"], "records": st["raw"]}
-
-        def fetch(self):
-            ks = list(self.acc)
-            return (np.array([self.code[k] for k in ks], dtype=np.uint64),
-                    np.array([self.acc[k] for k in ks], dtype=np.uint64), np.zeros(len(ks), dtype=np.uint64))
-
-        def fetch_words(self, tb, mode, width=32, with_codes=True):
-            ks = list(self.acc)
-            words = np.array([k[:width] for k in ks], dtype="S%d" % width) if ks else np.zeros(0, dtype="S%d" % width)
-            counts = np.array([self.acc[k] for k in ks], dtype=np.uint64)
-            if not with_codes:
-                return words, counts, None, None
-            codes = np.array([self.code[k] for k in ks], dtype=np.uint64)
-            reps = np.array([self.rep.get(k, 0) for k in ks], dtype=np.uint64)
-            return words, counts, codes, reps
-
-    class Ctx(FakeTextCtx):
-        live = None
-
-        def table(self, log2):
-            return FieldsTable(self, log2)
-
-        def kv(self, capacity):
-            return RecKV(self, capacity)
-
-        def mem_info(self):
-            return (free_bytes - sum(self.live.values()), 1 << 34)
-    c = Ctx()
-    c.live = {}
-    return c
-
-
-def run_ours(src, P, monkeypatch, ctx=None):
-    """records (sorted reprs) of pipeline src over path P and the stage strings of the run"""
-    from fake_device import FakePinned
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
-    monkeypatch.setattr(runner_mod, "_CTX", {settings.device: ctx or make_ctx()})
-    monkeypatch.setattr(plan, "_pinned_ring", lambda n, b: [FakePinned(b) for _ in range(n)])
-    monkeypatch.setattr(plan, "_BUFFERS", {})
-    got = sorted(repr(x) for x in eval(src, {"Dampr": Dampr, "P": P}).run())
-    return got, [h for _s, h, _d in runner_mod.LAST_STATS.stages], runner_mod.LAST_STATS.stages
-
-
 # ---- comparison -------------------------------------------------------------------------------------------------
-def python_lines(path):
-    """the reader's lines: text-mode files with universal newlines, .gz files split at '\\n' only"""
-    paths = [os.path.join(path, f) for f in sorted(os.listdir(path))] if os.path.isdir(path) else [path]
-    out = []
-    for p in paths:
-        if p.endswith(".gz"):
-            with gzip.open(p, "rb") as f:
-                out += [l.decode("utf-8").rstrip("\n") for l in f]
-        else:
-            with open(p) as f:
-                out += [l.rstrip("\n") for l in f]
-    return out
-
-
 def same_records(got, exp, path=None, key=None, value=None):
     """sorted reprs equal, floats within the sum bound of their key: 4 n 2^-53 Σ|v| (+ one rounding for a mean)"""
     g = [ast.literal_eval(x.replace("nan", "None").replace("inf", "1e999")) for x in got]
@@ -343,7 +102,7 @@ def _kv_fns(src):
 # ---- the matcher ------------------------------------------------------------------------------------------------
 def _spec(key, value, split=None):
     from dampr_b200 import lowering
-    return lowering.text_fields_value_spec(key, value, split)
+    return lowering.text_fields_spec(key, value, split)
 
 
 def _mean_value(value):
@@ -361,16 +120,19 @@ def test_matcher_accepts_float_values_and_means():
     assert _spec(lambda r: r[1], _mean_value(lambda r: int(r[2])), sp) == (",", 1, FIELD_STR, 2, FIELD_INT, True)
     assert _spec(lambda l: l.split(";")[0], _mean_value(lambda l: int(l.split(";")[3]))) == \
         (";", 0, FIELD_STR, 3, FIELD_INT, True)
+    # the int and count shapes of the same spec
+    assert _spec(lambda r: r[0], lambda r: int(r[1]), sp) == (",", 0, FIELD_STR, 1, FIELD_INT, False)
+    assert _spec(lambda r: r[0], lambda r: 1, sp) == (",", 0, FIELD_STR, None, FIELD_INT, False)
+    assert _spec(lambda r: r[0], lambda r: float(r[1]), sp) == (",", 0, FIELD_STR, 1, FIELD_FLOAT, False)
 
 
 def test_matcher_rejects_the_near_misses():
     sp = lambda l: l.split(",")
     for key, value, split in [
-        (lambda r: r[0], lambda r: int(r[1]), sp),                 # int values are text_fields_spec's
         (lambda r: float(r[0]), lambda r: float(r[1]), sp),        # float key
         (lambda r: r[0], lambda r: float(r[1].strip()), sp),
         (lambda r: r[0], lambda r: float(r[1]) * 2, sp),
-        (lambda r: r[0], lambda r: 1, sp),
+        (lambda r: r[0], _mean_value(lambda r: 1), sp),            # mean of a constant
         (lambda r: (r[0], r[1]), lambda r: float(r[2]), sp),       # tuple key
         (lambda r: r[0], _mean_value(lambda r: r[2]), sp),         # mean of a str
         (lambda r: r[0], _mean_value(lambda r: float(r)), sp),
@@ -381,15 +143,13 @@ def test_matcher_rejects_the_near_misses():
         (lambda r: r[0], _mean_value(lambda r, s=1: float(r[2])), sp),
     ]:
         assert _spec(key, value, split) is None, (key, value, split)
-    from dampr_b200 import lowering   # text_fields_spec itself still refuses float values
-    assert lowering.text_fields_spec(lambda r: r[0], lambda r: float(r[1]), sp) is None
 
 
 # ---- against the reference --------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name", sorted(datasets()))
 def test_float_folds_agree_with_the_reference(name, monkeypatch, tmp_path):
     files = datasets()[name]
-    exp = reference_outputs(files, PIPELINES[name])
+    exp = reference_outputs(files, PIPELINES[name], GOLDEN)
     P = write_files(tmp_path, files)
     for src, e in zip(PIPELINES[name], exp):
         got, hows, stages = run_ours(src, P, monkeypatch)
@@ -399,7 +159,7 @@ def test_float_folds_agree_with_the_reference(name, monkeypatch, tmp_path):
 
 
 def test_the_issue_example():
-    exp = reference_outputs(datasets()["issue"], PIPELINES["issue"])
+    exp = reference_outputs(datasets()["issue"], PIPELINES["issue"], GOLDEN)
     assert exp[1] == ["('a', 1.5)", "('b', 2.25)", "('c', 7.0)"]
 
 
@@ -409,6 +169,10 @@ def test_modes_are_named_in_the_stats(monkeypatch, tmp_path):
     for src, op in [(C4 + ".a_group_by(lambda r: r[0], lambda r: float(r[1])).sum()", "op=sum_f64"),
                     (C4 + ".a_group_by(lambda r: r[0], lambda r: float(r[1])).reduce(max)", "op=max_f64"),
                     (C4 + ".a_group_by(lambda r: r[0], lambda r: float(r[1])).reduce(min)", "op=min_f64"),
+                    (C4 + ".a_group_by(lambda r: r[0], lambda r: int(r[2])).sum()", "op=sum_i64"),
+                    (C4 + ".a_group_by(lambda r: r[0], lambda r: int(r[2])).reduce(max)", "op=max_i64"),
+                    (C4 + ".a_group_by(lambda r: r[0], lambda r: int(r[2])).reduce(min)", "op=min_i64"),
+                    ("Dampr.text(P).count(lambda l: l.split(',')[0])", "op=count"),
                     (C4 + ".mean(lambda r: r[0], lambda r: float(r[1]))", "op=mean_f64"),
                     (C4 + ".mean(lambda r: r[0], lambda r: int(r[2]))", "op=mean_i64")]:
         got, hows, stages = run_ours(src, P, monkeypatch)
