@@ -416,8 +416,10 @@ text_count_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, u6
                         break;
                     }
             }
-            if (dup) continue;
             bool hashed = (key >> 63) != 0;
+            // the de-dup compares codes only: the verify pass still byte-compares a hashed duplicate with the
+            // entry's representative, so a different word of the same code on the line sets TF_COLLISION
+            if (dup && !(VERIFY && hashed)) continue;
             if (VERIFY) {
                 if (hashed) {
                     u32 pos = s.tpos[t];

@@ -568,6 +568,8 @@ text_count2_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, u
                 bool dup = !valid;
                 if (MODE == DAMPR_TOK_NONWORD_LOWER_SET) {
 #if DAMPR_TEXT_USE_MATCH
+                    // (not built) merges equal codes here and in the combiner below without a byte compare: a
+                    // build of it must pass the code-collision tests before it is selected
                     u32 m1 = 0, m2 = 0;
                     if (valid) {
                         m1 = __match_any_sync(vmask, key);
@@ -656,16 +658,19 @@ text_count2_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, u
                 // verification.  str.split mode: 10+ byte tokens are common and Zipf-hot, so they go through
                 // the shared-memory combiner like the exact codes; an entry remembers the latest occurrence
                 // of its token and every hit is compared with it (bytes) before it is counted.
+                // set() de-duplication above compares codes only: a hashed token it dropped still goes to the
+                // table with count 0, so its bytes are compared with the entry's representative like any other
+                // and a different word of the same code sets TF_COLLISION instead of vanishing
                 u64 myrep = ~0ULL;
-                if (live && hashed) {
+                if (valid && hashed && (live || MODE == DAMPR_TOK_NONWORD_LOWER_SET)) {
                     u32 l2 = len;
                     if (l2 >= (1u << 20)) {
                         my_flags |= DAMPR_TF_LONGTOKEN;
                         l2 = (1u << 20) - 1;
                     }
                     myrep = ((base_offset + (sgl - V_LEAD) + pos) << 20) | l2;
-                    acc_long++;
-                    if (!WS && !hashed_insert(key, myrep, 1ULL)) my_flags |= DAMPR_TF_COLLISION;
+                    acc_long += live ? 1 : 0;
+                    if (!WS && !hashed_insert(key, myrep, live ? 1ULL : 0ULL)) my_flags |= DAMPR_TF_COLLISION;
                 }
                 const bool ins = live && (WS || !hashed);
                 const u32 imask = __ballot_sync(0xFFFFFFFFu, ins);
