@@ -9,8 +9,9 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdampr_b200.so")
 SOURCES = ["ctx.cu", "text.cu", "text2.cu", "fields.cu", "kv.cu", "merge.cu", "ops.cu", "comm.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+# host code: no contraction of a * b + c into one rounding (dampr_host_eval_f64 must round like CPython)
 NVCC_FLAGS = ARCH + [
-    "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+    "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-ffp-contract=off",
 ]
 
 

@@ -105,6 +105,9 @@ struct dampr_table {
     u64 cap;
     u64 *tiles;   // device: per-tile line counts / bases of dampr_text_fields_records (grown on demand)
     u64 tiles_cap;
+    u64 *ext;     // device: the count column of the last dampr_table_fetch_words, in its row order (grown on demand)
+    u64 ext_cap;
+    u64 ext_n;    // 0 after a clear
 };
 
 struct dampr_kv {

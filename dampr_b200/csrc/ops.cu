@@ -593,3 +593,88 @@ int32_t dampr_textbuf_download(dampr_ctx *ctx, dampr_textbuf *tb, uint64_t off, 
 }
 
 }  // extern "C"
+
+// ---- a lowered numeric lambda over the distinct values of an int64 column (host) ----------------------------------
+// The cross of a frame with a one-row broadcast evaluates the user's function once per distinct value of the field it
+// reads (plan._lower_cross). For expressions of + - * / neg, float() and math.log over that field, int and float
+// constants and the broadcast value, plan.py compiles the tree into this postfix program, typed the way CPython types
+// it. Every operation is the IEEE double operation CPython performs (the library is built without contraction or
+// fast-math, and log is the C library's, which math.log calls for a finite positive argument), so the results are
+// CPython's to the bit. Wherever CPython would raise or take another road (a zero divisor, a log argument that is not
+// finite and positive, an int leaving int64, an int true division beyond 2^53) the call returns
+// DAMPR_ERR_UNSUPPORTED and the caller evaluates the function in Python instead.
+#include <cmath>
+
+namespace {
+enum EvalOp : int32_t {
+    EV_X = 0,      // push the column value (int)
+    EV_CI = 1,     // push int constant ci[arg]
+    EV_CF = 2,     // push float constant cf[arg]
+    EV_I2F = 3,    // float() of the int on top
+    EV_IADD = 4, EV_ISUB = 5, EV_IMUL = 6,
+    EV_FADD = 7, EV_FSUB = 8, EV_FMUL = 9, EV_FDIV = 10,
+    EV_IDIV = 11,  // int / int: true division
+    EV_LOG = 12,   // math.log of the float on top
+    EV_INEG = 13, EV_FNEG = 14,
+};
+union EvalSlot {
+    long long i;
+    double f;
+};
+}  // namespace
+
+extern "C" int32_t dampr_host_eval_f64(const int64_t *vals, uint64_t n, const int32_t *prog, uint32_t prog_len,
+                                       const int64_t *ci, const double *cf, double *out) {
+    if ((!vals || !out) && n) return DAMPR_ERR_ARG;
+    if (!prog || prog_len == 0 || prog_len > 256) return DAMPR_ERR_ARG;
+    // the program is checked once: every operation finds its operands, one value is left
+    int depth = 0;
+    for (uint32_t pc = 0; pc < prog_len; ++pc) {
+        const int32_t op = prog[pc] & 0xFF;
+        const bool push = op <= EV_CF, unary = op == EV_I2F || op == EV_LOG || op == EV_INEG || op == EV_FNEG;
+        if (op > EV_FNEG || depth < (push ? 0 : unary ? 1 : 2)) return DAMPR_ERR_ARG;
+        depth += push ? 1 : unary ? 0 : -1;
+        if (depth > 64) return DAMPR_ERR_ARG;
+    }
+    if (depth != 1) return DAMPR_ERR_ARG;
+    const long long LIM53 = 1LL << 53;
+    EvalSlot st[64];
+    for (uint64_t r = 0; r < n; ++r) {
+        int sp = 0;
+        for (uint32_t pc = 0; pc < prog_len; ++pc) {
+            const int32_t op = prog[pc] & 0xFF, arg = prog[pc] >> 8;
+            EvalSlot &a = st[sp >= 2 ? sp - 2 : 0], &b = st[sp >= 1 ? sp - 1 : 0];
+            switch (op) {
+                case EV_X: st[sp++].i = vals[r]; break;
+                case EV_CI: st[sp++].i = ci[arg]; break;
+                case EV_CF: st[sp++].f = cf[arg]; break;
+                case EV_I2F: b.f = (double)b.i; break;
+                case EV_IADD: if (__builtin_add_overflow(a.i, b.i, &a.i)) return DAMPR_ERR_UNSUPPORTED; --sp; break;
+                case EV_ISUB: if (__builtin_sub_overflow(a.i, b.i, &a.i)) return DAMPR_ERR_UNSUPPORTED; --sp; break;
+                case EV_IMUL: if (__builtin_mul_overflow(a.i, b.i, &a.i)) return DAMPR_ERR_UNSUPPORTED; --sp; break;
+                case EV_FADD: a.f = a.f + b.f; --sp; break;
+                case EV_FSUB: a.f = a.f - b.f; --sp; break;
+                case EV_FMUL: a.f = a.f * b.f; --sp; break;
+                case EV_FDIV:
+                    if (b.f == 0.0) return DAMPR_ERR_UNSUPPORTED;
+                    a.f = a.f / b.f;
+                    --sp;
+                    break;
+                case EV_IDIV:
+                    if (b.i == 0 || a.i > LIM53 || a.i < -LIM53 || b.i > LIM53 || b.i < -LIM53) return DAMPR_ERR_UNSUPPORTED;
+                    a.f = (double)a.i / (double)b.i;
+                    --sp;
+                    break;
+                case EV_LOG:
+                    if (!(b.f > 0.0) || !std::isfinite(b.f)) return DAMPR_ERR_UNSUPPORTED;
+                    b.f = log(b.f);
+                    break;
+                case EV_INEG: if (b.i == INT64_MIN) return DAMPR_ERR_UNSUPPORTED; b.i = -b.i; break;
+                case EV_FNEG: b.f = -b.f; break;
+                default: return DAMPR_ERR_ARG;
+            }
+        }
+        out[r] = st[0].f;
+    }
+    return DAMPR_OK;
+}

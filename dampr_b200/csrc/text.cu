@@ -654,7 +654,8 @@ int32_t dampr_table_create(dampr_ctx *ctx, uint32_t capacity_log2, dampr_table *
     dampr_table *t = new dampr_table();
     t->cap_log2 = capacity_log2;
     t->cap = 1ULL << capacity_log2;
-    t->keys = t->counts = t->reps = t->stats = t->fb = t->tiles = nullptr;
+    t->keys = t->counts = t->reps = t->stats = t->fb = t->tiles = t->ext = nullptr;
+    t->ext_cap = t->ext_n = 0;
     t->fb_cap = 1u << 16;
     if (cudaMalloc(&t->keys, t->cap * 8) != cudaSuccess || cudaMalloc(&t->counts, t->cap * 8) != cudaSuccess ||
         cudaMalloc(&t->reps, t->cap * 8) != cudaSuccess || cudaMalloc(&t->stats, 8 * 8) != cudaSuccess ||
@@ -685,12 +686,14 @@ int32_t dampr_table_destroy(dampr_ctx *ctx, dampr_table *t) {
     cudaFree(t->stats);
     cudaFree(t->fb);
     cudaFree(t->tiles);
+    cudaFree(t->ext);
     delete t;
     return DAMPR_OK;
 }
 
 int32_t dampr_table_clear(dampr_ctx *ctx, dampr_table *t) {
     ARG_CHECK(ctx, ctx && t, "null");
+    t->ext_n = 0;
     {
         ScopedTimer tm(ctx, DAMPR_K_MISC);
         table_init_kernel<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(t->keys, t->counts, t->reps, t->cap,
@@ -888,13 +891,23 @@ extern "C" int32_t dampr_table_fetch_words(dampr_ctx *ctx, dampr_table *t, dampr
     if (!words) return DAMPR_OK;
     ARG_CHECK(ctx, cap >= st[0] && counts, "fetch arrays too small");   // codes / reps are optional
     u64 m = st[0];
+    t->ext_n = 0;
     if (m == 0) return DAMPR_OK;
-    u64 per = width + 24;
+    // the count column stays on the device (t->ext) for dampr_count_dictionary
+    if (t->ext_cap < m) {
+        CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+        cudaFree(t->ext);
+        t->ext = nullptr;
+        t->ext_cap = 0;
+        CUDA_TRY(ctx, cudaMalloc(&t->ext, m * 8));
+        t->ext_cap = m;
+    }
+    u64 per = width + 16;
     u8 *d = (u8 *)pool_alloc(ctx, m * per + 8);
     ARG_CHECK(ctx, d != nullptr, "device allocation failed");
     u8 *d_words = d;
-    u64 *d_counts = (u64 *)(d + m * width);
-    u64 *d_codes = d_counts + m;
+    u64 *d_counts = t->ext;
+    u64 *d_codes = (u64 *)(d + m * width);
     u64 *d_reps = d_codes + m;
     u64 *d_cur = d_reps + m;
     CUDA_TRY(ctx, cudaMemsetAsync(d_cur, 0, 8, ctx->stream));
@@ -918,7 +931,228 @@ extern "C" int32_t dampr_table_fetch_words(dampr_ctx *ctx, dampr_table *t, dampr
         ctx->err = std::string("table fetch_words failed: ") + cudaGetErrorString(e);
         return DAMPR_ERR_CUDA;
     }
+    if (rc2 == DAMPR_OK) t->ext_n = m;
     return rc2;
+}
+
+extern "C" int32_t dampr_table_extracted_counts(dampr_ctx *ctx, dampr_table *t, uint64_t *dev_ptr, uint64_t *n) {
+    ARG_CHECK(ctx, ctx && t && dev_ptr && n, "null");
+    *dev_ptr = (uint64_t)(uintptr_t)t->ext;
+    *n = t->ext_n;
+    return DAMPR_OK;
+}
+
+// ---- dictionary of a count column on the device ----------------------------------------------------------
+// Sorted distinct values, the inverse (uint32, row order) and the smallest row holding each value. Values below a
+// bound B go through a presence table: mark, count per 1024-entry block, scan the block counts, rank every present
+// value. The few values at or above B (the head of a Zipf count distribution) are sorted and folded by
+// dampr_kv_sort_reduce and found again by binary search. Row i < n reads counts[i * stride]; rows n.. are `extra`.
+namespace {
+
+constexpr u32 DICT_BLOCK = 1024;
+
+__device__ __forceinline__ u64 dict_value(const u64 *counts, u64 n, u32 stride, const u64 *extra, u64 i) {
+    return i < n ? counts[i * stride] : extra[i - n];
+}
+
+__global__ void dict_mark_kernel(const u64 *__restrict__ counts, u64 n, u32 stride, const u64 *__restrict__ extra,
+                                 u64 rows, u64 bound, u32 *__restrict__ flag, u32 *__restrict__ first,
+                                 ulonglong2 *__restrict__ big, u64 *__restrict__ ctr) {
+    for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < rows; i += (u64)gridDim.x * blockDim.x) {
+        const u64 v = dict_value(counts, n, stride, extra, i);
+        if (v < bound) {
+            if (!flag[v]) flag[v] = 1;
+            if (first[v] > (u32)i) atomicMin(&first[v], (u32)i);
+        } else {
+            if ((long long)v < 0) ctr[1] = 1;   // negative: the two ranges would interleave
+            const u64 s = atomicAdd((unsigned long long *)&ctr[0], 1ULL);
+            big[s] = make_ulonglong2(v, i);
+        }
+    }
+}
+
+__global__ void dict_block_count_kernel(const u32 *__restrict__ flag, u32 *__restrict__ bsum) {
+    const u32 present = __syncthreads_count(flag[blockIdx.x * (u64)DICT_BLOCK + threadIdx.x] != 0);
+    if (threadIdx.x == 0) bsum[blockIdx.x] = present;
+}
+
+// exclusive scan of nb <= 4 * DICT_BLOCK block counts in one block; bsum[nb] = total
+__global__ void dict_scan_kernel(u32 *__restrict__ bsum, u32 nb) {
+    __shared__ u32 s[DICT_BLOCK];
+    const u32 per = (nb + DICT_BLOCK - 1) / DICT_BLOCK;
+    const u32 lo = threadIdx.x * per, hi = min(nb, lo + per);
+    u32 acc = 0;
+    for (u32 j = lo; j < hi; ++j) acc += bsum[j];
+    s[threadIdx.x] = acc;
+    __syncthreads();
+    for (u32 d = 1; d < DICT_BLOCK; d <<= 1) {
+        const u32 x = threadIdx.x >= d ? s[threadIdx.x - d] : 0;
+        __syncthreads();
+        s[threadIdx.x] += x;
+        __syncthreads();
+    }
+    u32 run = s[threadIdx.x] - acc;
+    for (u32 j = lo; j < hi; ++j) {
+        const u32 c = bsum[j];
+        bsum[j] = run;
+        run += c;
+    }
+    if (threadIdx.x == DICT_BLOCK - 1) bsum[nb] = s[DICT_BLOCK - 1];
+}
+
+// flag[v] becomes the rank of v among the present values; uniq / rows receive v and its first row
+__global__ void dict_rank_kernel(u32 *__restrict__ flag, const u32 *__restrict__ first, const u32 *__restrict__ boff,
+                                 long long *__restrict__ uniq, u32 *__restrict__ rows) {
+    __shared__ u32 warp_tot[DICT_BLOCK / 32];
+    const u64 v = blockIdx.x * (u64)DICT_BLOCK + threadIdx.x;
+    const bool have = flag[v] != 0;
+    const u32 m = __ballot_sync(0xFFFFFFFFu, have);
+    const u32 lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    if (lane == 0) warp_tot[w] = __popc(m);
+    __syncthreads();
+    if (w == 0) {
+        const u32 x = warp_tot[lane];
+        u32 incl = x;
+        for (u32 d = 1; d < 32; d <<= 1) {
+            const u32 y = __shfl_up_sync(0xFFFFFFFFu, incl, d);
+            if (lane >= d) incl += y;
+        }
+        warp_tot[lane] = incl - x;
+    }
+    __syncthreads();
+    if (have) {
+        const u32 r = boff[blockIdx.x] + warp_tot[w] + __popc(m & ((1u << lane) - 1u));
+        flag[v] = r;
+        uniq[r] = (long long)v;
+        rows[r] = first[v];
+    }
+}
+
+__global__ void dict_inv_kernel(const u64 *__restrict__ counts, u64 n, u32 stride, const u64 *__restrict__ extra,
+                                u64 rows, u64 bound, const u32 *__restrict__ rank, u32 *__restrict__ inv) {
+    for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < rows; i += (u64)gridDim.x * blockDim.x) {
+        const u64 v = dict_value(counts, n, stride, extra, i);
+        if (v < bound) inv[i] = rank[v];
+    }
+}
+
+// the folded large values (key order) appended after the m_small ranked ones; the large rows' inverse by search
+__global__ void dict_big_kernel(const ulonglong2 *__restrict__ big, u64 nbig, const ulonglong2 *__restrict__ red,
+                                u64 nred, u32 m_small, long long *__restrict__ uniq, u32 *__restrict__ rows,
+                                u32 *__restrict__ inv) {
+    for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < nbig; i += (u64)gridDim.x * blockDim.x) {
+        if (i < nred) {
+            uniq[m_small + i] = (long long)red[i].x;
+            rows[m_small + i] = (u32)red[i].y;
+        }
+        const u64 v = big[i].x;
+        u64 lo = 0, hi = nred;
+        while (hi - lo > 1) {
+            const u64 mid = (lo + hi) >> 1;
+            if (red[mid].x <= v) lo = mid;
+            else hi = mid;
+        }
+        inv[big[i].y] = m_small + (u32)lo;
+    }
+}
+
+}  // namespace
+
+extern "C" int32_t dampr_count_dictionary(dampr_ctx *ctx, const uint64_t *counts, uint64_t n, uint32_t stride,
+                                          const int64_t *extra, uint32_t n_extra, int64_t *uniq, uint32_t *inv,
+                                          uint32_t *rows, uint64_t *n_uniq) {
+    ARG_CHECK(ctx, ctx && uniq && inv && rows && n_uniq && stride >= 1, "null");
+    ARG_CHECK(ctx, (counts || n == 0) && (extra || n_extra == 0), "null column");
+    const u64 N = n + n_extra;
+    ARG_CHECK(ctx, N < (1ULL << 32), "more than 2^32 rows");
+    const u64 *col = (const u64 *)counts;
+    *n_uniq = 0;
+    if (N == 0) return DAMPR_OK;
+    CtxScope scope_(ctx);
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    wait_uploads(ctx);
+    // the presence table is cleared and scanned once: proportional to the column, at most 2^22 entries
+    u64 B = 4096;
+    while (B < 2 * N && B < (1ULL << 22)) B <<= 1;
+    const u32 nb = (u32)(B / DICT_BLOCK);
+    // flag[B] first[B] bsum[nb + 1] | ctr[2] extra[n_extra] | uniq[N] | rows[N] inv[N] | big[N]
+    const u64 o_ctr = ((2 * B + nb + 1) * 4 + 15) & ~15ULL;
+    const u64 o_uniq = (o_ctr + 16 + n_extra * 8 + 15) & ~15ULL;
+    const u64 o_rows = o_uniq + N * 8;
+    const u64 o_inv = o_rows + N * 4;
+    const u64 o_big = (o_inv + N * 4 + 15) & ~15ULL;
+    DevBuf buf;
+    CUDA_TRY(ctx, buf.alloc(o_big + N * 16));
+    u8 *base = (u8 *)buf.p;
+    u32 *flag = (u32 *)base, *first = flag + B, *bsum = first + B;
+    u64 *ctr = (u64 *)(base + o_ctr);
+    u64 *d_extra = ctr + 2;
+    long long *d_uniq = (long long *)(base + o_uniq);
+    u32 *d_rows = (u32 *)(base + o_rows), *d_inv = (u32 *)(base + o_inv);
+    ulonglong2 *big = (ulonglong2 *)(base + o_big);
+    CUDA_TRY(ctx, cudaMemsetAsync(flag, 0, B * 4, ctx->stream));
+    CUDA_TRY(ctx, cudaMemsetAsync(first, 0xFF, B * 4, ctx->stream));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctr, 0, 16, ctx->stream));
+    if (n_extra) CUDA_TRY(ctx, cudaMemcpyAsync(d_extra, extra, n_extra * 8, cudaMemcpyHostToDevice, ctx->stream));
+    const int grid = ctx->num_sms * 4;
+    {
+        ScopedTimer tm(ctx, DAMPR_K_MISC);
+        dict_mark_kernel<<<grid, 256, 0, ctx->stream>>>(col, n, stride, d_extra, N, B, flag, first, big, ctr);
+    }
+    {
+        ScopedTimer tm(ctx, DAMPR_K_MISC);
+        dict_block_count_kernel<<<nb, DICT_BLOCK, 0, ctx->stream>>>(flag, bsum);
+    }
+    {
+        ScopedTimer tm(ctx, DAMPR_K_MISC);
+        dict_scan_kernel<<<1, DICT_BLOCK, 0, ctx->stream>>>(bsum, nb);
+    }
+    {
+        ScopedTimer tm(ctx, DAMPR_K_MISC);
+        dict_rank_kernel<<<nb, DICT_BLOCK, 0, ctx->stream>>>(flag, first, bsum, d_uniq, d_rows);
+    }
+    {
+        ScopedTimer tm(ctx, DAMPR_K_MISC);
+        dict_inv_kernel<<<grid, 256, 0, ctx->stream>>>(col, n, stride, d_extra, N, B, flag, d_inv);
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+    // how many values are large, whether one is negative, how many are small
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_scratch, ctr, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_scratch + 2, bsum + nb, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    const u64 nbig = ctx->h_scratch[0];
+    const bool negative = ctx->h_scratch[1] != 0;
+    const u32 m_small = (u32)(ctx->h_scratch[2] & 0xFFFFFFFFu);
+    if (negative) return set_err(ctx, DAMPR_ERR_UNSUPPORTED, "%s", "negative values in a count column");
+    u64 m = m_small;
+    if (nbig) {
+        dampr_kv *kv = nullptr, *red = nullptr;
+        int rc = dampr_kv_create(ctx, nbig, &kv);
+        if (rc) return rc;
+        cudaError_t e = cudaMemcpyAsync(kv->rec, big, nbig * 16, cudaMemcpyDeviceToDevice, ctx->stream);
+        kv->n = nbig;
+        rc = e == cudaSuccess ? dampr_kv_sort_reduce(ctx, kv, DAMPR_KEY_I64, DAMPR_OP_MIN_I64, &red)
+                              : set_err(ctx, DAMPR_ERR_CUDA, "%s", cudaGetErrorString(e));
+        if (rc == DAMPR_OK) {
+            {
+                ScopedTimer tm(ctx, DAMPR_K_MISC);
+                dict_big_kernel<<<(unsigned)((nbig + 255) / 256), 256, 0, ctx->stream>>>(big, nbig, red->rec, red->n, m_small,
+                                                                                       d_uniq, d_rows, d_inv);
+            }
+            m += red->n;
+            e = cudaGetLastError();
+            if (e != cudaSuccess) rc = set_err(ctx, DAMPR_ERR_CUDA, "%s", cudaGetErrorString(e));
+        }
+        dampr_kv_destroy(ctx, kv);
+        if (red) dampr_kv_destroy(ctx, red);
+        if (rc) return rc;
+    }
+    CUDA_TRY(ctx, cudaMemcpyAsync(inv, d_inv, N * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(uniq, d_uniq, m * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(rows, d_rows, m * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    *n_uniq = m;
+    return DAMPR_OK;
 }
 
 // ---- host-side sink formatting (SinkWriter, dataset.py:264-282: one print(value) per record) --------

@@ -125,6 +125,9 @@ def load_library():
     _sig(lib, "dampr_table_fetch", vp, vp, vp, vp, vp, u64, pu64)
     _sig(lib, "dampr_table_to_kv", vp, vp, pvp)
     _sig(lib, "dampr_table_fetch_words", vp, vp, vp, i32, u32, vp, vp, vp, vp, u64, pu64)
+    _sig(lib, "dampr_table_extracted_counts", vp, vp, pu64, pu64)
+    _sig(lib, "dampr_count_dictionary", vp, vp, u64, u32, vp, u32, vp, vp, vp, pu64)
+    _sig(lib, "dampr_host_eval_f64", vp, u64, vp, u32, vp, vp, vp)
     _sig(lib, "dampr_kv_decode_words", vp, vp, i32, u32, vp)
     _sig(lib, "dampr_host_join_tsv", u64, i32, vp, vp, vp, vp, vp, vp, u64, pu64)
     _sig(lib, "dampr_host_sink_tsv", C.c_char_p, C.c_uint32, C.c_uint32, u64, i32, vp, vp, vp, vp, vp, pu64,
@@ -383,6 +386,34 @@ class Ctx(object):
         self.sync()
         return kv
 
+    def count_dictionary(self, dev_ptr, n, stride=1, extra=()):
+        """(sorted distinct values int64, inverse uint32, smallest row of every value int64) of a non-negative
+        count column on the device (dampr_count_dictionary): rows 0..n-1 are the u64 values at dev_ptr (every
+        `stride`-th), then the host values `extra`. None when a value is negative."""
+        ex = np.ascontiguousarray(extra, dtype=np.int64)
+        N = int(n) + len(ex)
+        uniq = np.empty(max(1, N), dtype=np.int64)
+        inv = np.empty(N, dtype=np.uint32)
+        rows = np.empty(max(1, N), dtype=np.uint32)
+        m = C.c_uint64(0)
+        rc = self.lib.dampr_count_dictionary(self.h, C.c_void_p(int(dev_ptr)) if n else None, int(n), int(stride),
+                                             _ptr(ex) if len(ex) else None, len(ex), _ptr(uniq), _ptr(inv),
+                                             _ptr(rows), C.byref(m))
+        if rc == -5:   # DAMPR_ERR_UNSUPPORTED
+            return None
+        self.check(rc)
+        m = m.value
+        return uniq[:m], inv, rows[:m].astype(np.int64)
+
+    def count_dictionary_of(self, counts, extra=()):
+        """count_dictionary of a host column (uploaded as the values of a kv's records)"""
+        counts = np.ascontiguousarray(counts).view(np.uint64)
+        kv = self.kv_from_columns(np.zeros(len(counts), dtype=np.uint64), counts)
+        try:
+            return self.count_dictionary(kv.devptr() + 8, len(counts), 2, extra)
+        finally:
+            kv.free()
+
 
 class TextBuf(object):
     def __init__(self, ctx, capacity):
@@ -442,9 +473,17 @@ class Table(object):
         ctx.check(ctx.lib.dampr_table_create(ctx.h, int(capacity_log2), C.byref(h)))
         self.h = h
         self.capacity = 1 << capacity_log2
+        self.fetches = 0   # fetch_words / clear calls so far: tells whether extracted_counts() is still a given fetch's
 
     def clear(self):
+        self.fetches += 1
         self.ctx.check(self.ctx.lib.dampr_table_clear(self.ctx.h, self.h))
+
+    def extracted_counts(self):
+        """(device pointer, length) of the count column the last fetch_words downloaded, in its row order"""
+        p, n = C.c_uint64(0), C.c_uint64(0)
+        self.ctx.check(self.ctx.lib.dampr_table_extracted_counts(self.ctx.h, self.h, C.byref(p), C.byref(n)))
+        return p.value, n.value
 
     def count(self, tb, lo, hi, mode, cr_is_data=False):
         """cr_is_data: '\\r' is an ordinary byte (the reference's binary-mode .gz reader) instead of a line end"""
@@ -512,6 +551,7 @@ class Table(object):
     def fetch_words(self, tb, mode, width=32, with_codes=True):
         """(words 'S<width>' array decoded on the device, counts, codes, reps); codes and reps are None
         when with_codes is false (tables without hashed tokens need neither)."""
+        self.fetches += 1
         n = C.c_uint64(0)
         self.ctx.check(self.ctx.lib.dampr_table_fetch_words(self.ctx.h, self.h, None, int(mode), int(width), None,
                                                             None, None, None, 0, C.byref(n)))
@@ -797,6 +837,23 @@ def host_unique_small(col, table=1 << 20, with_rows=False):
             rb[il] = br
             rows = np.concatenate((rows, rb))
     return (uniq, inv, rows) if with_rows else (uniq, inv)
+
+
+def host_eval_f64(vals, prog, ci, cf):
+    """float64 result of a lowered numeric expression (lowering.numeric_program) at every value of an int64 array,
+    computed natively with CPython's rounding; None where CPython would raise or leave the IEEE path."""
+    lib = load_library()
+    vals = np.ascontiguousarray(vals, dtype=np.int64)
+    p = np.ascontiguousarray(prog, dtype=np.int32)
+    ci = np.ascontiguousarray(list(ci) or [0], dtype=np.int64)
+    cf = np.ascontiguousarray(list(cf) or [0.0], dtype=np.float64)
+    out = np.empty(len(vals), dtype=np.float64)
+    rc = lib.dampr_host_eval_f64(_ptr(vals), len(vals), _ptr(p), len(p), _ptr(ci), _ptr(cf), _ptr(out))
+    if rc == -5:   # DAMPR_ERR_UNSUPPORTED
+        return None
+    if rc:
+        raise DeviceError("dampr_host_eval_f64: malformed program (%d)" % rc)
+    return out
 
 
 def kv_merge_ranges(ctx, kv, offsets, xform, op=-1):

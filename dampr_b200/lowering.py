@@ -495,3 +495,99 @@ def depends_on(e, argi, fields=None):
         return all(walk(y) for y in (x.a, x.b, x.c) if y is not None)
 
     return out if walk(e) else None
+
+
+# ---- numeric expressions evaluated natively (dampr_host_eval_f64) -------------------------------------------------
+_EV = dict(X=0, CI=1, CF=2, I2F=3, IADD=4, ISUB=5, IMUL=6, FADD=7, FSUB=8, FMUL=9, FDIV=10, IDIV=11, LOG=12,
+           INEG=13, FNEG=14)
+_EV_BIN = {"+": ("IADD", "FADD"), "-": ("ISUB", "FSUB"), "*": ("IMUL", "FMUL")}
+
+
+def _callee(f):
+    """the Python object a call node calls: a global / builtin, or an attribute of one (math.log)"""
+    if isinstance(f, E) and f.op == "obj":
+        return f.a
+    if isinstance(f, E) and f.op == "attr" and isinstance(f.a, E) and f.a.op == "obj" and isinstance(f.b, str):
+        return getattr(f.a.a, f.b, None)
+    return None
+
+
+def numeric_program(e, field, scalar, argi=1):
+    """Postfix program of dampr_host_eval_f64 for a float-valued expression over one int64 field `field` of argument
+    `argi` (the column), the other argument as the broadcast value `scalar` (an int or a float) and int / float
+    constants, built from + - * /, unary -, float() and math.log — typed as CPython types it (int operands of a float
+    operation are converted first, int / int is true division). Returns (program, int constants, float constants),
+    or None for anything outside that set (the caller then calls the function in Python)."""
+    import math
+    prog, ci, cf = [], [], []
+
+    def num(v):
+        if type(v) is int:
+            if not -(1 << 63) <= v < (1 << 63):
+                return None
+            ci.append(v)
+            prog.append(_EV["CI"] | (len(ci) - 1) << 8)
+            return "i"
+        if type(v) is float:
+            cf.append(v)
+            prog.append(_EV["CF"] | (len(cf) - 1) << 8)
+            return "f"
+        return None
+
+    def to_float(t):
+        if t == "i":
+            prog.append(_EV["I2F"])
+        return "f" if t else None
+
+    def walk(x):
+        if not isinstance(x, E):
+            return None
+        if x.op == "sub" and _is_arg(x.a, argi):
+            ok, i = _const(x.b)
+            if ok and type(i) is int and i == field:
+                prog.append(_EV["X"])
+                return "i"
+            return None
+        if x.op == "arg":
+            return num(scalar) if x.a != argi else None
+        if x.op == "const":
+            return num(x.a)
+        if x.op == "neg":
+            t = walk(x.a)
+            if t:
+                prog.append(_EV["INEG" if t == "i" else "FNEG"])
+            return t
+        if x.op == "bin" and x.a in ("+", "-", "*", "/"):
+            tl = walk(x.b)
+            if not tl:
+                return None
+            at = len(prog)            # where the left operand's conversion goes, if the right one is a float
+            tr = walk(x.c)
+            if not tr:
+                return None
+            if x.a == "/" and tl == tr == "i":
+                prog.append(_EV["IDIV"])
+                return "f"
+            if tl == tr == "i":
+                prog.append(_EV[_EV_BIN[x.a][0]])
+                return "i"
+            if tl == "i":
+                prog.insert(at, _EV["I2F"])
+            to_float(tr)
+            prog.append(_EV["FDIV" if x.a == "/" else _EV_BIN[x.a][1]])
+            return "f"
+        if x.op == "call" and isinstance(x.b, tuple) and len(x.b) == 1:
+            f = _callee(x.a)
+            if f is float:
+                return to_float(walk(x.b[0]))
+            if f is math.log:
+                t = to_float(walk(x.b[0]))
+                if t:
+                    prog.append(_EV["LOG"])
+                return t
+        return None
+
+    t = walk(e)
+    if t != "f" or len(prog) > 256:
+        return None
+    return prog, ci, cf

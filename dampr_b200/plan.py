@@ -56,8 +56,33 @@ class DictCol(object):
         return [u[j] for j in il]
 
 
+# The dictionary of the count column of the last device text scan, built on the device when first asked for:
+# (the column object, a function returning (uniq, inv, rows) or None, its result once known)
+_COUNT_DICT = [None, None, None]
+
+
+def remember_count_dictionary(col, build):
+    _COUNT_DICT[:] = [col, build, None]
+
+
+def forget_count_dictionary():
+    _COUNT_DICT[:] = [None, None, None]
+
+
+def _known_dictionary(col):
+    if _COUNT_DICT[0] is not col:
+        return None
+    if _COUNT_DICT[2] is None and _COUNT_DICT[1] is not None:
+        build, _COUNT_DICT[1] = _COUNT_DICT[1], None
+        _COUNT_DICT[2] = build()
+    return _COUNT_DICT[2]
+
+
 def unique_inverse_rows(col):
     """unique_inverse plus one row index per distinct value (any row holding it)."""
+    known = _known_dictionary(col)
+    if known is not None:
+        return known
     n = len(col)
     if n >= 4096 and col.dtype == np.int64:
         r = dev.host_unique_small(col, with_rows=True)
@@ -72,6 +97,9 @@ def unique_inverse_rows(col):
 def unique_inverse(col):
     """(sorted unique values, inverse index uint32) of an int64/float64 column. Small non-negative
     ints (the bulk of count columns) go through a counting pass instead of a sort."""
+    known = _known_dictionary(col)
+    if known is not None:
+        return known[0], known[1]
     n = len(col)
     if n >= 4096 and col.dtype == np.int64:
         r = dev.host_unique_small(col)   # native presence-table pass; None if the values do not suit it
@@ -459,6 +487,7 @@ class TextScan(object):
         if flags & dev.TF_COLLISION:
             raise NotLowerable("64-bit key-code collision between two long tokens")
         words, counts = self._fetch_words(tab, tb, st, self.mode)
+        self._fetched = (getattr(tab, "fetches", None), len(counts))   # the table still holds this column on the device
         self.words = words
         self.counts = counts.view(np.int64)
         self.n_lines = int(st["lines"])
@@ -490,6 +519,19 @@ class TextScan(object):
                 wl[i] = s if mode == dev.TOK_WS else s.lower()
             words = wl
         return (words, counts, codes) if want_codes else (words, counts)
+
+    def count_dictionary(self, extra=()):
+        """unique_inverse_rows of the count column followed by the rows `extra`, computed on the device from the
+        column the table still holds; None when the table has moved on (another scan, another fetch) or host-
+        tokenised lines changed the column."""
+        tab = self._tab
+        fetched = getattr(self, "_fetched", None)
+        if tab is None or fetched is None or fetched[0] is None or fetched[0] != tab.fetches or self.host_lines:
+            return None
+        ptr, n = tab.extracted_counts()
+        if n != fetched[1]:
+            return None
+        return self.runner.ctx.count_dictionary(ptr, n, 1, extra)
 
     def _fallback_lines(self, tb, tab):
         """(offset, line) of every line on the table's fallback list, split by the reference's reader rules"""
@@ -1063,12 +1105,16 @@ def _lower_map(runner, stage, inputs, si):
         src, mode = m
         scan = text_scan(runner, src, mode)
         words, counts = scan.words, scan.counts
+        extra = []
         if mode != dev.TOK_WS and scan.empty:
             if isinstance(words, np.ndarray):
                 words = np.concatenate((words, np.array([b""], dtype=words.dtype)))
             else:
                 words = words + [""]
-            counts = np.concatenate((counts, np.array([scan.empty], dtype=np.int64)))
+            extra = [scan.empty]
+            counts = np.concatenate((counts, np.array(extra, dtype=np.int64)))
+        # a cross or a sink that dictionary-encodes this column gets the dictionary built on the device
+        remember_count_dictionary(counts, lambda: scan.count_dictionary(extra))
         f = Frame(words, [counts], scalar=True, combined=True)
         runner.stats.add(stage, "device text tokenise+combine",
                          "bytes=%d terms=%d lines=%d" % (scan.nbytes, len(words), scan.n_lines))
@@ -1768,15 +1814,15 @@ def _lower_cross(runner, stage, inputs):
         # decoding of thousands of keys nobody looks at). The user's function still evaluates its other
         # components on them; if one of those chokes on a placeholder the full rows are used instead.
         m = len(rep)
-        res = None
-        if pick is not None and len(outer.cols) > len(dep):
+        res = _native_eval(comp, dep[0], inner, uniq)
+        if res is None and pick is not None and len(outer.cols) > len(dep):
             try:
                 res = evaluate([_gather(c, rep) if j in dep else [None] * m for j, c in enumerate(outer.cols)])
             except Exception:
                 res = None
         if res is None:
             res = evaluate([_gather(c, rep) for c in outer.cols])
-        kinds = set(type(x) for x in res)
+        kinds = set(type(x) for x in res) if isinstance(res, list) else None
         if kinds == {float}:
             res = np.array(res, dtype=np.float64)
         elif kinds == {int}:
@@ -1786,6 +1832,18 @@ def _lower_cross(runner, stage, inputs):
     runner.stats.add(stage, "frame cross with a 1-row broadcast (memoised per distinct field value)",
                      "records=%d" % outer.n)
     return f
+
+
+def _native_eval(comp, field, inner, uniq):
+    """float64 values of one cross component at the distinct values `uniq` of the int field it reads, computed by
+    the library (dampr_host_eval_f64, CPython's results to the bit), or None: the component is outside the lowered
+    numeric set (lowering.numeric_program), or CPython would raise or leave the IEEE path for some value."""
+    if not (isinstance(uniq, np.ndarray) and uniq.dtype == np.int64):
+        return None
+    prog = lowering.numeric_program(comp, field, inner)
+    if prog is None:
+        return None
+    return dev.host_eval_f64(uniq, *prog)
 
 
 def _gather(col, idx):

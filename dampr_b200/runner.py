@@ -136,6 +136,7 @@ class B200Runner(object):
             self.stats.ms.append((str(stage.output), 1e3 * (time.perf_counter() - t_stage)))
             if not isinstance(stage, GSink):
                 produced.append(stage.output)
+        plan.forget_count_dictionary()
         ret = []
         keep = set()
         for src in outputs:

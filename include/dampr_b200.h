@@ -232,6 +232,18 @@ int32_t dampr_table_fetch(dampr_ctx *ctx, dampr_table *t, uint64_t *codes, uint6
 int32_t dampr_table_fetch_words(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, int32_t mode,
                                 uint32_t width, uint8_t *words, uint64_t *counts, uint64_t *codes,
                                 uint64_t *reps, uint64_t cap, uint64_t *n);
+/* device pointer and length of the count column the last dampr_table_fetch_words downloaded, in the same row
+ * order; it stays valid until the table is cleared, fetched again or destroyed (*n = 0 after a clear) */
+int32_t dampr_table_extracted_counts(dampr_ctx *ctx, dampr_table *t, uint64_t *dev_ptr, uint64_t *n);
+/* dictionary encoding of a non-negative count column ON THE DEVICE: row i < n holds counts[i * stride] (a device
+ * array; stride 2 reads the values of a kv's records at devptr + 8), rows n .. n + n_extra - 1 hold the host values
+ * extra[]. Writes the sorted distinct values uniq[0 .. *n_uniq), inv[i] (their index, per row) and rows[j] (the
+ * smallest row holding uniq[j]); every output array holds n + n_extra entries. Values below a bound are ranked
+ * through a presence table, the few above it are folded by dampr_kv_sort_reduce. A negative value returns
+ * DAMPR_ERR_UNSUPPORTED. n + n_extra < 2^32. */
+int32_t dampr_count_dictionary(dampr_ctx *ctx, const uint64_t *counts, uint64_t n, uint32_t stride,
+                               const int64_t *extra, uint32_t n_extra, int64_t *uniq, uint32_t *inv,
+                               uint32_t *rows, uint64_t *n_uniq);
 /* the same decoding for a kv whose keys are token codes (an exchanged / merged run): exact codes ->
  * words_host[i*width ..], hashed codes -> all-NUL (the caller patches them from their strings) */
 int32_t dampr_kv_decode_words(dampr_ctx *ctx, dampr_kv *kv, int32_t mode, uint32_t width,
@@ -271,6 +283,14 @@ int32_t dampr_host_sink_fmt(const char *prefix, uint32_t first_index, uint32_t m
 int32_t dampr_host_unique_small(const int64_t *col, uint64_t n, uint64_t table, int64_t *uniq,
                                 uint64_t *n_uniq, uint32_t *inv, uint32_t *first_row, int64_t *big_vals,
                                 uint64_t *big_rows, uint64_t big_cap, uint64_t *n_big);
+/* out[r] = a lowered numeric expression of vals[r] (host): prog is postfix, one int32 per operation, the opcode in
+ * the low byte and the constant's index above it — 0 push vals[r], 1 push ci[idx], 2 push cf[idx], 3 float() of an
+ * int, 4/5/6 int + - *, 7/8/9/10 float + - * /, 11 int / int (true division), 12 math.log, 13 int negation,
+ * 14 float negation. CPython's results to the bit; DAMPR_ERR_UNSUPPORTED where CPython would raise or leave the
+ * IEEE path (zero divisor, log of a value that is not finite and positive, int64 overflow, int / int beyond 2^53),
+ * DAMPR_ERR_ARG for a malformed program. */
+int32_t dampr_host_eval_f64(const int64_t *vals, uint64_t n, const int32_t *prog, uint32_t prog_len,
+                            const int64_t *ci, const double *cf, double *out);
 /* same, but leaves the run on the device as a kv (key = code, val = count) */
 int32_t dampr_table_to_kv(dampr_ctx *ctx, dampr_table *t, dampr_kv **out);
 
