@@ -33,6 +33,13 @@
 // (the same kernel, COUNT mode, sharing the line-start code) writes the lines per tile, one CTA scans them into
 // tile bases and advances run_base (a table stats slot), then the fold pass writes the records. No CTA waits for
 // another, and the records of a scan do not depend on how it is cut into ranges.
+//
+// WHERE (the stage's `filter(...)` calls, a compile-time parameter, so the plain scans compile as before): up to 8
+// predicates travel in the kernel's parameters (WhereView, ~1.6 KB, read in place through __grid_constant__).
+// Predicate j owns bound slot j; the separator walk that finds the key and value also finds every predicate's
+// field, the slots unrolled at compile time so the bounds stay in registers. The predicates are then evaluated in
+// chain order: the first false one drops the line before its key or value is parsed (a hole in record mode); one
+// the device cannot decide sends the line to the host, whose Python filters decide or raise.
 #include "common.cuh"
 #include "fparse.cuh"
 
@@ -52,8 +59,10 @@ static_assert(TEXT_LEAD >= F_LEAD, "textbuf lead-in too small");
 static_assert(TEXT_TAIL_PAD >= F_WIN + 64, "textbuf tail pad too small");
 static_assert(TEXT_TAIL_PAD >= (int)F_FB_MAXLEN + 1, "tail pad must cover the long-line measurement");
 
-// S_RECORDS: record mode's running record count (run_base of the next range)
+// S_RECORDS: record mode's running record count (run_base of the next range); S_DROPPED: the same slot in table
+// mode, the lines a WHERE predicate rejected
 enum { S_ENTRIES = 0, S_LINES = 1, S_MAXABS = 2, S_FOLDED = 3, S_FLAGS = 4, S_LONG = 5, S_RECORDS = 6, S_FALLBACK = 7 };
+enum { S_DROPPED = S_RECORDS };
 
 enum { VK_INT = 0, VK_F64 = 1 };                      // value kind: int() or float()
 enum { M_TABLE = 0, M_COUNT = 1, M_RECORDS = 2 };     // fold into the table / count lines per tile / write records
@@ -81,6 +90,23 @@ struct FieldsView {
     int op;
     u32 cr_is_data;
 };
+
+constexpr int P_MAX = DAMPR_PRED_MAX;
+
+struct PredSlot {
+    int field;           // index into the split line (negative from the end); unused for NFIELDS
+    u8 kind, cmp;        // DAMPR_PRED_*, DAMPR_CMP_*
+    u8 first, n;         // constants c[first, first + n)
+};
+
+// the predicates of a WHERE scan, passed by value in the kernel parameters (4 KB limit)
+struct WhereView {
+    PredSlot p[P_MAX];
+    long long c[DAMPR_PRED_MAX_CONSTS];   // INT / NFIELDS values, the bits of an F64 constant, STR: offset << 32 | len
+    u8 b[DAMPR_PRED_MAX_BYTES];           // STR constants
+    int n;
+};
+static_assert(sizeof(WhereView) + 256 <= 4096, "kernel parameters");
 
 struct SmemF {
     alignas(16) u8 text[F_WIN];
@@ -123,6 +149,62 @@ __device__ __forceinline__ bool parse_int(const u8 *p, u32 len, long long &out) 
     }
     out = neg ? -v : v;
     return true;
+}
+
+// c = sign of (field - constant) under an ordered comparison EQ .. GE
+__device__ __forceinline__ bool cmp_holds(int cmp, int c) {
+    switch (cmp) {
+        case DAMPR_CMP_EQ: return c == 0;
+        case DAMPR_CMP_NE: return c != 0;
+        case DAMPR_CMP_LT: return c < 0;
+        case DAMPR_CMP_LE: return c <= 0;
+        case DAMPR_CMP_GT: return c > 0;
+        default: return c >= 0;
+    }
+}
+
+// byte order of the field p[0, len) against STR constant k (UTF-8 byte order is code-point order, as Python's)
+__device__ __forceinline__ int str_order(const WhereView &w, const u8 *p, u32 len, long long k) {
+    const u8 *s = w.b + (k >> 32);
+    const u32 kl = (u32)k;
+    const u32 m = min(len, kl);
+    for (u32 i = 0; i < m; ++i)
+        if (p[i] != s[i]) return p[i] < s[i] ? -1 : 1;
+    return len < kl ? -1 : (len > kl ? 1 : 0);
+}
+
+// one predicate over its field p[0, len) (nf: the line's field count): 1 true, 0 false, -1 for the host to decide
+// (no such field, or an int() / float() field the device does not parse exactly)
+__device__ __noinline__ int eval_pred(const WhereView &w, const PredSlot &pr, bool has, const u8 *p, u32 len,
+                                      int nf) {
+    if (pr.kind == DAMPR_PRED_NFIELDS) return cmp_holds(pr.cmp, nf < w.c[pr.first] ? -1 : nf > w.c[pr.first]);
+    if (!has) return -1;   // IndexError in Python
+    const bool in = pr.cmp == DAMPR_CMP_IN || pr.cmp == DAMPR_CMP_NOT_IN;
+    bool r = false;
+    if (pr.kind == DAMPR_PRED_F64) {
+        double x;
+        if (!parse_f64(p, len, x)) return -1;
+        const double k = __longlong_as_double(w.c[pr.first]);
+        switch (pr.cmp) {   // IEEE comparisons: NaN is false under all but !=, -0.0 == 0.0, as in Python
+            case DAMPR_CMP_EQ: return x == k;
+            case DAMPR_CMP_NE: return x != k;
+            case DAMPR_CMP_LT: return x < k;
+            case DAMPR_CMP_LE: return x <= k;
+            case DAMPR_CMP_GT: return x > k;
+            default: return x >= k;
+        }
+    }
+    if (pr.kind == DAMPR_PRED_INT) {
+        long long x;
+        if (!parse_int(p, len, x)) return -1;
+        if (!in) return cmp_holds(pr.cmp, x < w.c[pr.first] ? -1 : x > w.c[pr.first]);
+        for (int i = pr.first; i < pr.first + pr.n && !r; ++i) r = x == w.c[i];
+    } else {
+        if (!in) return cmp_holds(pr.cmp, str_order(w, p, len, w.c[pr.first]));
+        for (int i = pr.first; i < pr.first + pr.n && !r; ++i)
+            r = (u32)w.c[i] == len && str_order(w, p, len, w.c[i]) == 0;
+    }
+    return r == (pr.cmp == DAMPR_CMP_IN);
 }
 
 __device__ __forceinline__ u64 hash_bytes(const u8 *p, u32 len, u64 seed) {
@@ -220,9 +302,10 @@ __global__ void __launch_bounds__(SCAN_THREADS) fields_tile_scan_kernel(u64 *til
     if (tid == 0) *run = carry;
 }
 
-template <int VK, int MODE>
-__global__ void __launch_bounds__(F_THREADS)
-text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv) {
+// the kernel body over the tiles of [own_lo, own_hi); where: the predicates of a WHERE scan
+template <int VK, int MODE, bool WHERE>
+__device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi,
+                                             const FieldsView &tab, const RecView &rv, const WhereView *where) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SmemF &s = *reinterpret_cast<SmemF *>(smem_raw);
     const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -231,6 +314,7 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
     if (tid == 0) s.flags = 0;
 
     u64 acc_lines = 0, acc_long = 0, acc_maxabs = 0;
+    u64 acc_dropped = 0;   // WHERE: lines a predicate rejected
     u32 my_flags = 0;
 
     for (u64 tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -340,6 +424,7 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
             if (end >= lim) end = 0xFFFFFFFFu;   // the newline is at or past lim: not handled here
             const u64 gq = sgl - F_LEAD + q;     // global offset of the line
             bool to_host = bad || end == 0xFFFFFFFFu;
+            bool dropped = false;   // WHERE: a predicate is false
             long long val = 1, kval = 0;
             u64 code = 0, rep = ~0ULL;
             if (!to_host) {
@@ -348,13 +433,32 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
                 const int ki = tab.key_field < 0 ? tab.key_field + nf : tab.key_field;
                 const bool one = tab.val_field == DAMPR_FIELD_VAL_ONE;
                 const int vi = one ? 0 : (tab.val_field < 0 ? tab.val_field + nf : tab.val_field);
-                if (ki < 0 || ki >= nf || vi < 0 || vi >= nf) {
+                const bool kv_missing = ki < 0 || ki >= nf || vi < 0 || vi >= nf;
+                if (!WHERE && kv_missing) {
                     to_host = true;   // IndexError: Python raises it
                 } else {
                     // pass 2: field bounds (a separator at window position p closes field f and opens f + 1)
                     u32 ks = (ki == 0) ? q : 0xFFFFFFFFu, ke = (ki == nf - 1) ? end : 0xFFFFFFFFu;
                     u32 vs = (vi == 0) ? q : 0xFFFFFFFFu, ve = (vi == nf - 1) ? end : 0xFFFFFFFFu;
-                    const int need = max(ki, vi) + 1;   // separators to visit
+                    int need = max(ki, vi) + 1;   // separators to visit
+                    // WHERE: predicate j's field is pi[j] (-1: none, IndexError in Python), its bounds [ps[j], pe[j])
+                    int pi[WHERE ? P_MAX : 1];
+                    u32 ps[WHERE ? P_MAX : 1], pe[WHERE ? P_MAX : 1];
+                    if constexpr (WHERE) {
+                        const WhereView &wh = *where;
+#pragma unroll
+                        for (int j = 0; j < P_MAX; ++j) {
+                            int i = -1;
+                            if (j < wh.n && wh.p[j].kind != DAMPR_PRED_NFIELDS) {
+                                i = wh.p[j].field < 0 ? wh.p[j].field + nf : wh.p[j].field;
+                                if (i >= nf) i = -1;
+                            }
+                            pi[j] = i < 0 ? -1 : i;
+                            ps[j] = pi[j] == 0 ? q : 0xFFFFFFFFu;
+                            pe[j] = pi[j] == nf - 1 ? end : 0xFFFFFFFFu;
+                            need = max(need, pi[j] + 1);
+                        }
+                    }
                     int f = 0;
                     skip = q & 3u;
                     for (p4 = q & ~3u; f < need && p4 < end; p4 += 4) {
@@ -371,31 +475,62 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
                             if (p >= end) break;
                             if (f == ki) ke = p;
                             if (f == vi) ve = p;
+                            if constexpr (WHERE) {
+#pragma unroll
+                                for (int j = 0; j < P_MAX; ++j)
+                                    if (f == pi[j]) pe[j] = p;
+                            }
                             ++f;
                             if (f == ki) ks = p + 1;
                             if (f == vi) vs = p + 1;
+                            if constexpr (WHERE) {
+#pragma unroll
+                                for (int j = 0; j < P_MAX; ++j)
+                                    if (f == pi[j]) ps[j] = p + 1;
+                            }
                         }
                     }
-                    const u32 klen = ke - ks;
-                    if constexpr (VK == VK_F64) {
-                        double d;
-                        if (parse_f64(s.text + vs, ve - vs, d)) val = __double_as_longlong(d);
-                        else to_host = true;
-                    } else if (!one && !parse_int(s.text + vs, ve - vs, val)) {
-                        to_host = true;
+                    if constexpr (WHERE) {
+                        // chain order: the first false predicate drops the line, the first undecided one (and a
+                        // missing key or value field behind predicates that all hold) is the host's
+                        const WhereView &wh = *where;
+                        int verdict = 1;
+#pragma unroll
+                        for (int j = 0; j < P_MAX; ++j)
+                            if (j < wh.n && verdict == 1)
+                                verdict = eval_pred(wh, wh.p[j], pi[j] >= 0, s.text + ps[j], pe[j] - ps[j], nf);
+                        dropped = verdict == 0;
+                        to_host = verdict < 0 || (verdict == 1 && kv_missing);
                     }
-                    if (!to_host) {
-                        if (tab.key_int) {
-                            if (!parse_int(s.text + ks, klen, kval)) to_host = true;
-                            else code = (u64)kval ^ 0x8000000000000000ULL;
-                        } else if (klen >= 1 && klen <= 9) {
-                            for (int i = (int)klen - 1; i >= 0; --i) code = (code << 7) | s.text[ks + i];
-                        } else {
-                            code = hash_bytes(s.text + ks, klen, tab.seed);
-                            rep = ((sgl - F_LEAD + ks) << 20) | klen;
-                            acc_long++;
+                    if (!WHERE || !(to_host || dropped)) {
+                        const u32 klen = ke - ks;
+                        if constexpr (VK == VK_F64) {
+                            double d;
+                            if (parse_f64(s.text + vs, ve - vs, d)) val = __double_as_longlong(d);
+                            else to_host = true;
+                        } else if (!one && !parse_int(s.text + vs, ve - vs, val)) {
+                            to_host = true;
+                        }
+                        if (!to_host) {
+                            if (tab.key_int) {
+                                if (!parse_int(s.text + ks, klen, kval)) to_host = true;
+                                else code = (u64)kval ^ 0x8000000000000000ULL;
+                            } else if (klen >= 1 && klen <= 9) {
+                                for (int i = (int)klen - 1; i >= 0; --i) code = (code << 7) | s.text[ks + i];
+                            } else {
+                                code = hash_bytes(s.text + ks, klen, tab.seed);
+                                rep = ((sgl - F_LEAD + ks) << 20) | klen;
+                                acc_long++;
+                            }
                         }
                     }
+                }
+            }
+            if constexpr (WHERE) {
+                if (dropped) {   // the host's filters would drop it too: it goes nowhere
+                    acc_dropped++;
+                    if constexpr (MODE == M_RECORDS) put_record(rv, tbase + li, 0, 0, my_flags);   // a hole
+                    continue;
                 }
             }
             if (to_host) {
@@ -453,27 +588,91 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
         if (acc_long) atomicAdd(&tab.stats[S_LONG], acc_long);
         if (acc_maxabs) atomicMax(&tab.stats[S_MAXABS], acc_maxabs);
     }
+    if constexpr (WHERE && MODE == M_TABLE) {   // record mode: records - folded - fallback
+#pragma unroll
+        for (int d = 16; d > 0; d >>= 1) acc_dropped += __shfl_down_sync(0xFFFFFFFFu, acc_dropped, d);
+        if (lane == 0 && acc_dropped) atomicAdd(&tab.stats[S_DROPPED], acc_dropped);
+    }
     if (my_flags) atomicOr(&s.flags, my_flags);
     __syncthreads();
     if (tid == 0 && s.flags) atomicOr(&tab.stats[S_FLAGS], (u64)s.flags);
 }
 
-// one kernel over the tiles of [own_lo, own_hi)
-template <int VK, int MODE>
+// the plain scan (WHERE false) and the WHERE scan, whose predicates are read in place from the parameters
+template <int VK, int MODE, bool WHERE>
+__global__ void __launch_bounds__(F_THREADS)
+text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv) {
+    static_assert(!WHERE, "a WHERE scan takes its predicates");
+    fields_tiles<VK, MODE, false>(text, n, own_lo, own_hi, tab, rv, nullptr);
+}
+
+template <int VK, int MODE, bool WHERE>
+__global__ void __launch_bounds__(F_THREADS)
+text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv,
+                   const __grid_constant__ WhereView where) {
+    static_assert(WHERE, "a plain scan takes no predicates");
+    fields_tiles<VK, MODE, true>(text, n, own_lo, own_hi, tab, rv, &where);
+}
+
+// one kernel over the tiles of [own_lo, own_hi); WHERE: the build that applies the predicates *wh
+template <int VK, int MODE, bool WHERE = false>
 int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const FieldsView &tv, const RecView &rv,
-                  int timer) {
+                  int timer, const WhereView *wh = nullptr) {
     const size_t smem = sizeof(SmemF);
-    CUDA_TRY(ctx, cudaFuncSetAttribute(text_fields_kernel<VK, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)smem));
     const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
     u64 grid = (u64)ctx->num_sms * 4;
     if (grid > ntiles) grid = ntiles;
-    {
+    if constexpr (WHERE) {
+        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, WhereView) = text_fields_kernel<VK, MODE, true>;
+        CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         ScopedTimer tm(ctx, timer);
-        text_fields_kernel<VK, MODE><<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi,
-                                                                                        tv, rv);
+        kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *wh);
+    } else {
+        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView) = text_fields_kernel<VK, MODE, false>;
+        CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ScopedTimer tm(ctx, timer);
+        kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv);
     }
     CUDA_TRY(ctx, cudaGetLastError());
+    return DAMPR_OK;
+}
+
+// the predicates of spec in kernel-parameter form; DAMPR_ERR_ARG for a kind, comparison or limit outside the header's
+int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, WhereView &w) {
+    ARG_CHECK(ctx, spec->npreds >= 0 && spec->npreds <= DAMPR_PRED_MAX, "npreds must be 0 .. DAMPR_PRED_MAX");
+    ARG_CHECK(ctx, spec->npreds == 0 || spec->preds != nullptr, "null preds");
+    w = WhereView{};
+    w.n = spec->npreds;
+    int nc = 0, nb = 0;
+    for (int j = 0; j < spec->npreds; ++j) {
+        const dampr_field_pred &p = spec->preds[j];
+        const bool in = p.cmp == DAMPR_CMP_IN || p.cmp == DAMPR_CMP_NOT_IN;
+        ARG_CHECK(ctx, p.kind >= DAMPR_PRED_STR && p.kind <= DAMPR_PRED_NFIELDS, "predicate kind");
+        ARG_CHECK(ctx, p.cmp >= DAMPR_CMP_EQ && p.cmp <= DAMPR_CMP_NOT_IN, "predicate comparison");
+        ARG_CHECK(ctx, !in || p.kind == DAMPR_PRED_STR || p.kind == DAMPR_PRED_INT, "IN / NOT_IN take STR or INT");
+        ARG_CHECK(ctx, in ? (p.n >= 1 && p.n <= DAMPR_PRED_MAX_CONSTS) : p.n == 1, "predicate constant count");
+        ARG_CHECK(ctx, nc + p.n <= DAMPR_PRED_MAX_CONSTS, "more than DAMPR_PRED_MAX_CONSTS predicate constants");
+        w.p[j] = PredSlot{p.field, (u8)p.kind, (u8)p.cmp, (u8)nc, (u8)p.n};
+        for (int i = 0; i < p.n; ++i, ++nc) {
+            if (p.kind == DAMPR_PRED_F64) {
+                long long bits;
+                memcpy(&bits, &p.f64, sizeof bits);
+                w.c[nc] = bits;
+            } else if (p.kind == DAMPR_PRED_STR) {
+                ARG_CHECK(ctx, p.bytes != nullptr && p.lens != nullptr, "null predicate strings");
+                ARG_CHECK(ctx, p.lens[i] <= (uint32_t)(DAMPR_PRED_MAX_BYTES - nb),
+                          "more than DAMPR_PRED_MAX_BYTES bytes of predicate strings");
+                u32 off = 0;
+                for (int k = 0; k < i; ++k) off += p.lens[k];
+                if (p.lens[i]) memcpy(w.b + nb, p.bytes + off, p.lens[i]);
+                w.c[nc] = ((long long)nb << 32) | p.lens[i];
+                nb += (int)p.lens[i];
+            } else {
+                ARG_CHECK(ctx, p.ints != nullptr, "null predicate constants");
+                w.c[nc] = p.ints[i];
+            }
+        }
+    }
     return DAMPR_OK;
 }
 
@@ -485,13 +684,24 @@ int check_fields_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own
     ARG_CHECK(ctx, spec->sep > 0 && spec->sep < 0x80 && spec->sep != '\n' && spec->sep != '\r',
               "separator must be an ASCII byte other than NUL, '\\n' and '\\r'");
     ARG_CHECK(ctx, spec->key_kind == DAMPR_FIELD_KEY_STR || spec->key_kind == DAMPR_FIELD_KEY_INT, "key kind");
-    return DAMPR_OK;
+    WhereView w;
+    return where_view(ctx, spec, w);
 }
 
 FieldsView fields_view(dampr_table *t, const dampr_fields_spec *spec, int op) {
     return FieldsView{t->keys, t->counts, t->reps, t->stats, t->fb, t->cap - 1, 0x243F6A8885A308D3ULL, t->fb_cap,
                       (u32)spec->sep, spec->key_field, spec->val_field, spec->key_kind == DAMPR_FIELD_KEY_INT ? 1 : 0,
                       op, spec->cr_is_data ? 1u : 0u};
+}
+
+// the fold pass of one range: the plain kernel, or its WHERE build when spec holds predicates
+template <int VK, int MODE>
+int launch_fold(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
+                const FieldsView &tv, const RecView &rv) {
+    if (spec->npreds == 0) return launch_fields<VK, MODE>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS);
+    WhereView w;
+    if (int r = where_view(ctx, spec, w)) return r;
+    return launch_fields<VK, MODE, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w);
 }
 
 }  // namespace
@@ -507,8 +717,8 @@ extern "C" int32_t dampr_text_fields(dampr_ctx *ctx, dampr_table *t, dampr_textb
     if (own_hi <= own_lo) return DAMPR_OK;
     const FieldsView tv = fields_view(t, spec, spec->op);
     wait_uploads(ctx);
-    if (f64) return launch_fields<VK_F64, M_TABLE>(ctx, tb, own_lo, own_hi, tv, RecView{}, DAMPR_K_TEXT_FIELDS);
-    return launch_fields<VK_INT, M_TABLE>(ctx, tb, own_lo, own_hi, tv, RecView{}, DAMPR_K_TEXT_FIELDS);
+    if (f64) return launch_fold<VK_F64, M_TABLE>(ctx, tb, own_lo, own_hi, spec, tv, RecView{});
+    return launch_fold<VK_INT, M_TABLE>(ctx, tb, own_lo, own_hi, spec, tv, RecView{});
 }
 
 extern "C" int32_t dampr_text_fields_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
@@ -537,7 +747,6 @@ extern "C" int32_t dampr_text_fields_records(dampr_ctx *ctx, dampr_table *t, dam
         fields_tile_scan_kernel<<<1, SCAN_THREADS, 0, ctx->stream>>>(t->tiles, ntiles, t->stats + S_RECORDS);
     }
     CUDA_TRY(ctx, cudaGetLastError());
-    if (spec->op == DAMPR_OP_SUM_F64)
-        return launch_fields<VK_F64, M_RECORDS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS);
-    return launch_fields<VK_INT, M_RECORDS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS);
+    if (spec->op == DAMPR_OP_SUM_F64) return launch_fold<VK_F64, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, tv, rv);
+    return launch_fold<VK_INT, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, tv, rv);
 }

@@ -32,6 +32,10 @@ TOK_FLAG_CR_DATA = 0x100
 FIELD_KEY_STR, FIELD_KEY_INT = 0, 1
 FIELD_VAL_ONE = 0x7FFFFFFF
 FIELDS_HALO = 65536
+# WHERE predicates of a field scan (dampr_field_pred): kinds, comparisons, limits per call
+PRED_STR, PRED_INT, PRED_F64, PRED_NFIELDS = range(4)
+CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_IN, CMP_NOT_IN = range(8)
+PRED_MAX, PRED_MAX_CONSTS, PRED_MAX_BYTES = 8, 64, 1024
 
 KERNEL_NAMES = {
     1: "text_count", 2: "table_extract", 3: "text_verify", 4: "part_hist", 5: "part_scatter",
@@ -54,10 +58,44 @@ def decode_fold(acc, op):
     return acc.view(np.int64)
 
 
+class FieldPred(C.Structure):
+    """dampr_field_pred"""
+    _fields_ = [("kind", C.c_int32), ("field", C.c_int32), ("cmp", C.c_int32), ("n", C.c_int32),
+                ("ints", C.POINTER(C.c_int64)), ("f64", C.c_double), ("bytes", C.POINTER(C.c_uint8)),
+                ("lens", C.POINTER(C.c_uint32))]
+
+
 class FieldsSpec(C.Structure):
     """dampr_fields_spec"""
     _fields_ = [("sep", C.c_int32), ("key_field", C.c_int32), ("key_kind", C.c_int32), ("val_field", C.c_int32),
-                ("op", C.c_int32), ("cr_is_data", C.c_int32)]
+                ("op", C.c_int32), ("cr_is_data", C.c_int32), ("preds", C.POINTER(FieldPred)), ("npreds", C.c_int32)]
+
+
+def fields_spec(spec, cr_is_data, preds):
+    """dampr_fields_spec of spec = (sep byte, key field, key kind, value field or FIELD_VAL_ONE, op) and the WHERE
+    predicates preds = [(PRED_*, field, CMP_*, constants)]: constants a tuple of str (PRED_STR), int (PRED_INT,
+    PRED_NFIELDS) or one float (PRED_F64). The returned structure keeps its constant arrays alive."""
+    sep, kf, kind, vf, op = spec
+    arr = (FieldPred * max(1, len(preds)))()
+    keep = [arr]
+    for p, (pk, field, cmp, consts) in zip(arr, preds):
+        p.kind, p.field, p.cmp, p.n = int(pk), int(field), int(cmp), len(consts)
+        if pk == PRED_F64:
+            p.f64 = float(consts[0])
+        elif pk == PRED_STR:
+            raw = [c.encode("utf-8") for c in consts]
+            b = (C.c_uint8 * max(1, sum(map(len, raw)))).from_buffer_copy(b"".join(raw).ljust(1, b"\0"))
+            ln = (C.c_uint32 * len(raw))(*map(len, raw))
+            p.bytes, p.lens = C.cast(b, C.POINTER(C.c_uint8)), C.cast(ln, C.POINTER(C.c_uint32))
+            keep += [b, ln]
+        else:
+            v = (C.c_int64 * len(consts))(*map(int, consts))
+            p.ints = C.cast(v, C.POINTER(C.c_int64))
+            keep.append(v)
+    s = FieldsSpec(int(sep), int(kf), int(kind), int(vf), int(op), 1 if cr_is_data else 0,
+                   C.cast(arr, C.POINTER(FieldPred)), len(preds))
+    s._keep = keep
+    return s
 
 
 class DeviceError(RuntimeError):
@@ -490,24 +528,25 @@ class Table(object):
         m = int(mode) | (TOK_FLAG_CR_DATA if cr_is_data else 0)
         self.ctx.check(self.ctx.lib.dampr_text_count(self.ctx.h, self.h, tb.h, int(lo), int(hi), m))
 
-    def fields(self, tb, lo, hi, spec, cr_is_data=False):
+    def fields(self, tb, lo, hi, spec, cr_is_data=False, preds=()):
         """Fold the delimited fields of the lines starting in [lo, hi): spec = (sep byte, key field, key kind,
-        value field or FIELD_VAL_ONE, op); bytes up to hi + FIELDS_HALO must be uploaded."""
-        sep, kf, kind, vf, op = spec
-        s = FieldsSpec(int(sep), int(kf), int(kind), int(vf), int(op), 1 if cr_is_data else 0)
+        value field or FIELD_VAL_ONE, op); bytes up to hi + FIELDS_HALO must be uploaded. preds: the WHERE
+        predicates (see fields_spec), applied in order before the key and value are read."""
+        s = fields_spec(spec, cr_is_data, preds)
         self.ctx.check(self.ctx.lib.dampr_text_fields(self.ctx.h, self.h, tb.h, int(lo), int(hi), C.byref(s)))
 
-    def fields_records(self, tb, lo, hi, spec, kv, cr_is_data=False):
+    def fields_records(self, tb, lo, hi, spec, kv, cr_is_data=False, preds=()):
         """Record mode of fields() (spec op OP_SUM_I64 or OP_SUM_F64): one {key code, value} record per line starting
-        in [lo, hi) into kv's buffer, in line order, holes {0, 0} for the lines left to the host; the table counts
-        the lines per key. fields_stats()["records"] is the scan's record count (kv's size is the caller's)."""
-        sep, kf, kind, vf, op = spec
-        s = FieldsSpec(int(sep), int(kf), int(kind), int(vf), int(op), 1 if cr_is_data else 0)
+        in [lo, hi) into kv's buffer, in line order, holes {0, 0} for the lines left to the host or dropped by preds;
+        the table counts the lines per key. fields_stats()["records"] is the scan's record count (kv's size is the
+        caller's)."""
+        s = fields_spec(spec, cr_is_data, preds)
         self.ctx.check(self.ctx.lib.dampr_text_fields_records(self.ctx.h, self.h, tb.h, int(lo), int(hi), C.byref(s),
                                                               kv.h))
 
     def fields_stats(self):
-        """stats() of a field scan under the names of its counters"""
+        """stats() of a field scan under the names of its counters. "records" is the record count in record mode;
+        in table mode it counts the lines WHERE predicates dropped (record mode: records - lines - fallback)."""
         st = self.stats()
         return {"entries": st["entries"], "lines": st["lines"], "max_abs": st["empty"], "folded": st["folded"],
                 "flags": st["flags"], "hashed": st["hashed"], "fallback": st["fallback"], "records": st["raw"]}

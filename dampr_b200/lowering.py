@@ -322,6 +322,86 @@ def text_fields_spec(key_fn, value_fn, split_fn=None):
     return k[2], k[1], k[0], v[1], v[0], mean
 
 
+FIELD_COUNT = "nfields"
+_FLIP = {"==": "==", "!=": "!=", "<": ">", "<=": ">=", ">": "<", ">=": "<="}
+PRED_MAX, PRED_MAX_CONSTS, PRED_MAX_BYTES = 8, 64, 1024   # the device's limits per stage (include/dampr_b200.h)
+
+
+def _pred_const(e):
+    """(True, value) for a constant or a closure / global object"""
+    if isinstance(e, E) and e.op in ("const", "obj"):
+        return True, e.a
+    return False, None
+
+
+def field_predicate(fn, record=None):
+    """Device WHERE predicate of a `filter(fn)` in front of a field fold, or None. `record` is None when fn takes the
+    text line and splits it itself (l.split(S)), else the separator S of the map(lambda l: l.split(S)) fn runs after.
+    Returns (sep, kind, index, op, constants), with R the split record, for
+      F op C, C op F   F = R[i] (FIELD_STR), int(R[i]) (FIELD_INT) or float(R[i]) (FIELD_FLOAT), op one of
+                       == != < <= > >= (C op F comes back as F op' C); C a str for a str field, an int in int64 (not a
+                       bool) for an int field, a float or an int with |C| <= 2^53 (returned as a float) for a float
+                       field
+      F in K, F not in K   F = R[i] or int(R[i]); K a tuple / frozenset / set / list, literal or bound to a closure or
+                       global name (the members are read now), of 1 .. PRED_MAX_CONSTS members that are all str (a str
+                       field) or all int in int64 (an int field); constants is K's members
+      len(R) op n      kind FIELD_COUNT, index None, n an int (not a bool)
+    Everything else (and / or / not, chained comparisons, methods, raw-line tests, mixed types) is None."""
+    if not (isinstance(fn, types.FunctionType) and fn.__code__.co_argcount == 1):
+        return None
+    e = analyze(fn)
+    if e is None or e.op != "cmp":
+        return None
+    if record is None:
+        rec = _split_sep
+    else:
+        def rec(x):
+            return record if _is_arg(x) else None
+    op, l, r = e.a, e.b, e.c
+    if op in _FLIP and _pred_const(l)[0] and not _pred_const(r)[0]:
+        op, l, r = _FLIP[op], r, l
+    ok, c = _pred_const(r)
+    if not ok:
+        return None
+    if isinstance(l, E) and l.op == "call" and isinstance(l.a, E) and l.a.op == "obj" and l.a.a is len \
+            and len(l.b) == 1:
+        sep = rec(l.b[0])
+        if sep is None or op not in _FLIP or type(c) is not int:
+            return None
+        return sep, FIELD_COUNT, None, op, (c,)
+    p = _value_proj(l, rec) or _field_proj(l, rec)
+    if p is None:
+        return None
+    kind, i, sep = p
+    if op in ("in", "not in"):
+        if kind == FIELD_FLOAT or type(c) not in (tuple, frozenset, set, list) or \
+                not 1 <= len(c) <= PRED_MAX_CONSTS:
+            return None
+        consts = tuple(c)
+    elif op in _FLIP:
+        consts = (c,)
+    else:
+        return None
+    if kind == FIELD_STR:
+        if not all(type(m) is str for m in consts):
+            return None
+        try:
+            if sum(len(m.encode("utf-8")) for m in consts) > PRED_MAX_BYTES:
+                return None
+        except UnicodeEncodeError:   # a lone surrogate: no UTF-8 bytes to compare
+            return None
+    elif kind == FIELD_INT:
+        if not all(type(m) is int and -(1 << 63) <= m < (1 << 63) for m in consts):
+            return None
+    else:
+        v = consts[0]
+        if type(v) is int and abs(v) <= (1 << 53):
+            consts = (float(v),)
+        elif type(v) is not float:
+            return None
+    return sep, kind, i, op, consts
+
+
 def field_index(fn):
     """i if fn is `lambda x: x[i]` with a constant non-negative int i, else None."""
     e = analyze(fn)

@@ -748,9 +748,12 @@ class FieldScan(TextScan):
     HALO = dev.FIELDS_HALO   # a line longer than the kernel's window is measured up to 64 KB past its start
     REC_BYTES = 32           # per record: the record and the sort's scratch copy
 
-    def __init__(self, runner, sources, spec, op, stage, mean):
+    def __init__(self, runner, sources, spec, op, stage, mean, preds=()):
         TextScan.__init__(self, runner, sources, None)
         self.spec = spec     # (separator byte, key index, key kind, value index or FIELD_VAL_ONE)
+        self.preds = preds   # the stage's filters as device WHERE predicates (device.fields_spec)
+        self._where = {"preds": preds} if preds else {}
+        self.filtered = 0    # lines the predicates dropped on the device
         self.op = op
         self.stage = stage
         self.mean = mean     # values are mean()'s (sum, count) pairs
@@ -765,13 +768,14 @@ class FieldScan(TextScan):
     def _launch(self, tab, tb, lo, hi):
         spec = tuple(self.spec) + (self.op,)
         if not self.records:
-            tab.fields(tb, lo, hi, spec, getattr(self, "_cr_is_data", False))
+            # a stage without filters makes exactly the plain call
+            tab.fields(tb, lo, hi, spec, getattr(self, "_cr_is_data", False), **self._where)
             return
         if self._rec is None:
             # a first guess of one record per 32 bytes of text; a scan with more lines is repeated once with a
             # buffer of the exact size (DAMPR_TF_RECFULL)
             self._records_buffer(min(tb.n // 32 + 4096, self._free_bytes() // (2 * self.REC_BYTES)))
-        tab.fields_records(tb, lo, hi, spec, self._rec, getattr(self, "_cr_is_data", False))
+        tab.fields_records(tb, lo, hi, spec, self._rec, getattr(self, "_cr_is_data", False), **self._where)
 
     def _free_bytes(self):
         return int(self.runner.ctx.mem_info()[0])
@@ -853,6 +857,8 @@ class FieldScan(TextScan):
         self.groups = len(self.keys)
         self.n_lines = int(st["lines"]) + nrec   # one record per line
         self.host_lines = nrec
+        if self.preds:   # the table-mode slot, or the records that are neither folded nor handed back
+            self.filtered = int(st["records"]) - (int(st["lines"]) + int(st["fallback"]) if self.records else 0)
         return self
 
     def _record_sums(self, codes, n):
@@ -1013,24 +1019,38 @@ def _match_text_count(stage, inputs):
 
 
 def _match_text_fields(stage, inputs):
-    """[map(l.split(S)) ->] keyed(field key, 1 | int(field) | float(field)) + PartialReduceCombiner(+ | min | max),
-    or mean()'s keyed(field key, (int(field) | float(field), 1)) + component-wise (+, +), over text:
-    (sources, (sep byte, key index, key kind, value index or FIELD_VAL_ONE), op, mean) or None"""
+    """filter* [map(l.split(S)) filter*] keyed(field key, 1 | int(field) | float(field)) + PartialReduceCombiner(+ |
+    min | max), or mean()'s keyed(field key, (int(field) | float(field), 1)) + component-wise (+, +), over text, each
+    filter one lowering.field_predicate on the key's separator: (sources, (sep byte, key index, key kind, value index
+    or FIELD_VAL_ONE), op, mean, device predicates) or None"""
     if not isinstance(stage, GMap) or len(inputs) != 1:
         return None
     src = _text_files(inputs[0])
     if src is None:
         return None
     ks = _opkinds(stage.mapper)
-    if ks is None or [k for k, _ in ks] not in (["keyed"], ["map", "keyed"]):
+    kinds = [k for k, _ in ks] if ks is not None else []
+    if not kinds or kinds[-1] != "keyed" or any(k not in ("filter", "map") for k in kinds[:-1]) or \
+            kinds.count("map") > 1:
         return None
     if not isinstance(stage.combiner, ops.PartialReduceCombiner):
         return None
     keyed = ks[-1][1]
-    spec = lowering.text_fields_spec(keyed.fn, keyed.fn2, ks[0][1].fn if len(ks) == 2 else None)
+    at = kinds.index("map") if "map" in kinds else None
+    spec = lowering.text_fields_spec(keyed.fn, keyed.fn2, ks[at][1].fn if at is not None else None)
     if spec is None:
         return None
     sep, ki, kkind, vi, vkind, mean = spec
+    preds = []
+    for i, (k, o) in enumerate(ks[:-1]):
+        if k == "filter":
+            p = lowering.field_predicate(o.fn, sep if at is not None and i > at else None)
+            if p is None or p[0] != sep:
+                return None
+            preds.append(_device_pred(p))
+    if len(preds) > dev.PRED_MAX or sum(len(p[3]) for p in preds) > dev.PRED_MAX_CONSTS or \
+            sum(len(c.encode("utf-8")) for p in preds if p[0] == dev.PRED_STR for c in p[3]) > dev.PRED_MAX_BYTES:
+        return None
     binop = stage.options.get("binop")
     if mean:
         if lowering.tuple_binop_kinds(binop) != [lowering.ADD, lowering.ADD]:
@@ -1042,7 +1062,19 @@ def _match_text_fields(stage, inputs):
             return None
         op = (_FOLD_OPS_F64 if vkind == lowering.FIELD_FLOAT else _FOLD_OPS)[kind]
     return src, (ord(sep), ki, dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR,
-                 dev.FIELD_VAL_ONE if vi is None else vi), op, mean
+                 dev.FIELD_VAL_ONE if vi is None else vi), op, mean, tuple(preds)
+
+
+_PRED_KINDS = {lowering.FIELD_STR: dev.PRED_STR, lowering.FIELD_INT: dev.PRED_INT, lowering.FIELD_FLOAT: dev.PRED_F64,
+               lowering.FIELD_COUNT: dev.PRED_NFIELDS}
+_PRED_CMPS = {"==": dev.CMP_EQ, "!=": dev.CMP_NE, "<": dev.CMP_LT, "<=": dev.CMP_LE, ">": dev.CMP_GT, ">=": dev.CMP_GE,
+              "in": dev.CMP_IN, "not in": dev.CMP_NOT_IN}
+
+
+def _device_pred(p):
+    """(PRED_*, field, CMP_*, constants) of a lowering.field_predicate"""
+    _sep, kind, i, op, consts = p
+    return _PRED_KINDS[kind], 0 if i is None else i, _PRED_CMPS[op], consts
 
 
 _FIELD_OP_NAMES = {dev.OP_SUM_I64: "sum_i64", dev.OP_MIN_I64: "min_i64", dev.OP_MAX_I64: "max_i64",
@@ -1123,13 +1155,15 @@ def _lower_map(runner, stage, inputs, si):
     if m is not None:
         if dist.active():
             raise NotLowerable("the field scan runs on one process")
-        src, spec, op, mean = m
-        scan = FieldScan(runner, src, spec, op, stage, mean).run()
+        src, spec, op, mean, preds = m
+        scan = FieldScan(runner, src, spec, op, stage, mean, preds).run()
         opname = ("mean_f64" if op == dev.OP_SUM_F64 else "mean_i64") if mean else \
             "count" if spec[3] == dev.FIELD_VAL_ONE and op == dev.OP_SUM_I64 else _FIELD_OP_NAMES[op]
-        runner.stats.add(stage, "device text fields scan+combine",
-                         "op=%s bytes=%d lines=%d groups=%d host_lines=%d" % (opname, scan.nbytes, scan.n_lines,
-                                                                             scan.groups, scan.host_lines))
+        detail = "op=%s bytes=%d lines=%d groups=%d host_lines=%d" % (opname, scan.nbytes, scan.n_lines, scan.groups,
+                                                                      scan.host_lines)
+        if preds:
+            detail += " filtered=%d" % scan.filtered
+        runner.stats.add(stage, "device text fields scan+combine", detail)
         return Frame(scan.keys, [scan.values], scalar=True, combined=True)
     if _match_line_count(stage, inputs):
         ds = inputs[0]

@@ -174,6 +174,33 @@ int32_t dampr_table_fallback_lines(dampr_ctx *ctx, dampr_table *t, uint64_t *lin
 /* bytes past own_hi that must be uploaded before a dampr_text_fields call (a line longer than the kernel's window
  * is measured in global memory, up to 64 KB) */
 #define DAMPR_FIELDS_HALO 65536
+/* a WHERE predicate of a field scan: the stage's `filter(...)` calls in front of the fold, e.g. r[1] == 'GET',
+ * int(r[2]) >= 500, float(r[3]) < 0.5, r[1] in ('GET', 'POST'), len(r) == 4 (r = line.split(sep)) */
+#define DAMPR_PRED_STR 0      /* line.split(sep)[field], compared as bytes (UTF-8 byte order is code-point order)  */
+#define DAMPR_PRED_INT 1      /* int(line.split(sep)[field]) against int64 constants                               */
+#define DAMPR_PRED_F64 2      /* float(line.split(sep)[field]) against one double (IEEE: NaN is unequal to all)    */
+#define DAMPR_PRED_NFIELDS 3  /* len(line.split(sep)) against one int64; `field` is unused                        */
+#define DAMPR_CMP_EQ 0
+#define DAMPR_CMP_NE 1
+#define DAMPR_CMP_LT 2
+#define DAMPR_CMP_LE 3
+#define DAMPR_CMP_GT 4
+#define DAMPR_CMP_GE 5
+#define DAMPR_CMP_IN 6        /* STR and INT only: equal to one of the n constants                                */
+#define DAMPR_CMP_NOT_IN 7
+#define DAMPR_PRED_MAX 8              /* predicates per call                                                      */
+#define DAMPR_PRED_MAX_CONSTS 64      /* constants (set members included) over all predicates of a call           */
+#define DAMPR_PRED_MAX_BYTES 1024     /* bytes of STR constants over all predicates of a call                     */
+typedef struct dampr_field_pred {
+    int32_t kind;           /* DAMPR_PRED_*                                                                       */
+    int32_t field;          /* i of line.split(sep)[i]; negative counts from the end, as in Python                */
+    int32_t cmp;            /* DAMPR_CMP_*                                                                        */
+    int32_t n;              /* constants: 1 for EQ .. GE, 1 .. DAMPR_PRED_MAX_CONSTS members for IN / NOT_IN      */
+    const int64_t *ints;    /* INT, NFIELDS: the n constants                                                      */
+    double f64;             /* F64: the constant                                                                  */
+    const uint8_t *bytes;   /* STR: the n constants back to back                                                  */
+    const uint32_t *lens;   /* STR: their lengths in bytes                                                        */
+} dampr_field_pred;
 typedef struct dampr_fields_spec {
     int32_t sep;        /* separator byte: ASCII, not NUL, '\n' or '\r'                                     */
     int32_t key_field;  /* i of line.split(sep)[i]; negative counts from the end, as in Python              */
@@ -184,7 +211,17 @@ typedef struct dampr_fields_spec {
                            DAMPR_OP_MIN_F64 | MAX_F64 (float() values); dampr_text_fields_records:
                            DAMPR_OP_SUM_I64 (int() values) | DAMPR_OP_SUM_F64 (float() values)               */
     int32_t cr_is_data; /* 1: '\r' is an ordinary byte (binary-mode .gz); 0: it ends lines (text mode)        */
+    const dampr_field_pred *preds; /* WHERE predicates, applied in order before the key and value are read       */
+    int32_t npreds;     /* 0 .. DAMPR_PRED_MAX; 0 (preds unused) is the plain scan                                */
 } dampr_fields_spec;
+/* WHERE (npreds > 0): on each line the device can take (the byte and length rules below), the predicates are
+ * evaluated in order as Python's filters would be. The first false one drops the line: no key or value is read,
+ * nothing is inserted, record mode writes a hole {0, 0}, and the line goes nowhere else. A predicate the device
+ * cannot decide (its field does not exist, an INT field that is not [+-]?[0-9]{1,18}, an F64 field outside the
+ * float() rule below) hands the line to the caller as a fallback line, whose filters then decide or raise. Only a
+ * line that passes every predicate has its key and value read, under the rules below. A -0.0 in a predicate's field
+ * does not set DAMPR_TF_NEGZERO. Dropped lines are counted: dampr_text_fields puts their number in stats[6];
+ * in record mode it is stats[6] - stats[1] - stats[7] (records - folded lines - fallback lines). */
 /* fold (key code -> value) of the lines whose first byte lies in [own_lo, own_hi) into the table (cleared by the
  * caller before the first range; ranges of one scan accumulate). Needs bytes [0, min(n, own_hi + DAMPR_FIELDS_HALO))
  * uploaded. The device folds a line only when every byte is ASCII and not NUL, it holds no '\r' (unless

@@ -6,13 +6,21 @@ from CUDA events (dampr_ctx_timings, DAMPR_K_TEXT_FIELDS) with its GB/s and shar
 page-cache-warm file, the host-map MB/s on a sample, and whether the device and the host results agree there.
 
     python tools/fields_bench.py [--gb 2] [--keys 1000000] [--reps 3] [--sample-mb 32] [--out DIR]
-                                 [--value int|float] [--op sum|min|max|mean]
+                                 [--value int|float] [--op sum|min|max|mean] [--where none|str|int|float|set]
 
 --value float writes the value field as float text (even lines "%.6f", odd lines repr() of the double, right-aligned
 in a 24-byte field) and folds float(r[2]); --op picks `+` (fold_by), min / max (a_group_by().reduce) or mean(). A run
 other than the default also reports every kernel's time by name (the record modes' count pass, fold and sort), and
 for float sums and means whether the sample agrees with Python within 4·n·2^-53·Σ|v| per key (plus one rounding for
 a mean); the default run prints exactly the fields it always printed.
+
+--where adds one `filter` in front of the fold and runs the stage both ways in the same invocation: the unfiltered
+figures under their usual names, the filtered ones as where_* (kernel ms and GB/s over the same bytes, end-to-end
+MB/s, the stats line with filtered=N, and whether the host-map sample of the filtered stage agrees). The filters:
+  str    r[0] < 'u0500000'        (about half the lines at the default --keys)
+  int    int(r[2]) >= 0           (the signed value field: about half; --value int only)
+  float  float(r[2]) >= 0         (about half)
+  set    r[0] not in <64 keys>    (keeps almost every line: each one is compared with all 64 members)
 """
 import argparse
 import json
@@ -78,9 +86,16 @@ def float_text(seed, n_lines, n_keys):
     return out.reshape(-1)
 
 
-def job(Dampr, src, value="int", op="sum"):
+SET_KEYS = tuple("u%07d" % (i * 7919) for i in range(64))
+WHERE = {"str": lambda r: r[0] < "u0500000", "int": lambda r: int(r[2]) >= 0, "float": lambda r: float(r[2]) >= 0,
+         "set": lambda r: r[0] not in SET_KEYS}
+
+
+def job(Dampr, src, value="int", op="sum", where="none"):
     conv = int if value == "int" else float
     d = Dampr.read_input(src).map(lambda l: l.split(","))
+    if where != "none":
+        d = d.filter(WHERE[where])
     if op == "mean":
         return d.mean(lambda r: r[0], lambda r: conv(r[2]))
     if op in ("min", "max"):
@@ -88,12 +103,15 @@ def job(Dampr, src, value="int", op="sum"):
     return d.fold_by(lambda r: r[0], value=lambda r: conv(r[2]), binop=lambda a, b: a + b)
 
 
-def python_fold(sample, value, op):
+def python_fold(sample, value, op, where="none"):
     """the stage as plain Python over the sample's lines: {key: result}"""
     conv = int if value == "int" else float
+    keep = WHERE.get(where, lambda r: True)
     out = {}
     for l in sample.decode("ascii").split("\n")[:-1]:
         r = l.split(",")
+        if not keep(r):
+            continue
         k, v = r[0], conv(r[2])
         if op == "mean":
             s, n = out.get(k, (0, 0))
@@ -149,7 +167,10 @@ def main():
     ap.add_argument("--out", default=None, help="directory for the text file (default: a temporary one)")
     ap.add_argument("--value", choices=("int", "float"), default="int")
     ap.add_argument("--op", choices=("sum", "min", "max", "mean"), default="sum")
+    ap.add_argument("--where", choices=("none", "str", "int", "float", "set"), default="none")
     a = ap.parse_args()
+    if a.where == "int" and a.value != "int":
+        ap.error("--where int needs --value int (int() of a float field raises)")
     default = a.value == "int" and a.op == "sum"
 
     from dampr_b200 import Dampr, device as dev, plan
@@ -166,10 +187,10 @@ def main():
     text.tofile(path)
     del text
 
-    def timed(src):
+    def timed(src, where="none"):
         ctx.timings_reset()
         t0 = time.perf_counter()
-        n = len(list(job(Dampr, src, a.value, a.op).run()))
+        n = len(list(job(Dampr, src, a.value, a.op, where).run()))
         dt = time.perf_counter() - t0
         stages = runner_mod.LAST_STATS.stages
         assert "device text fields scan+combine" in stages[0][1], stages
@@ -188,6 +209,10 @@ def main():
             pass
     from dampr_b200.inputs import PathInput
     fil = [timed(PathInput(path)) for _ in range(a.reps)]
+    if a.where != "none":
+        timed(plan.MemoryText(pin.array), a.where)
+        wmem = [timed(plan.MemoryText(pin.array), a.where) for _ in range(a.reps)]
+        wfil = [timed(PathInput(path), a.where) for _ in range(a.reps)]
     ctx.timing_enable(False)
 
     # host map on a sample: the stage as plain Python (the same lambdas), and the device result of the same bytes
@@ -231,6 +256,24 @@ def main():
                     "kernels_ms": {k: round(v, 3) for k, v in sorted(best[4].items())}})
         if a.value == "float" and a.op in ("sum", "mean"):
             res["sample_within_bound"] = within_bound(got, host, magnitudes(sample), a.op)
+    if a.where != "none":
+        t0 = time.perf_counter()
+        whost = python_fold(sample, a.value, a.op, a.where)
+        whost_s = time.perf_counter() - t0
+        wgot = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op, a.where).run())
+        wk = min(m[1] for m in wmem)
+        res.update({
+            "where": a.where,
+            "where_kernel_ms": round(wk, 3),
+            "where_kernel_GBps": round(nbytes / wk / 1e6, 1),
+            "where_e2e_pinned_MBps": round(nbytes / min(m[0] for m in wmem) / 1e6, 1),
+            "where_e2e_pinned_s": [round(m[0], 3) for m in wmem],
+            "where_e2e_file_warm_MBps": round(nbytes / min(f[0] for f in wfil) / 1e6, 1),
+            "where_host_map_MBps": round(len(sample) / whost_s / 1e6, 1),
+            "where_sample_equal": wgot == whost if not (a.value == "float" and a.op in ("sum", "mean")) else
+            within_bound(wgot, whost, magnitudes(sample), a.op),
+            "where_stats": wmem[0][3],
+        })
     if a.out is None:
         shutil.rmtree(tmpdir, ignore_errors=True)
     print(json.dumps(res))
