@@ -71,7 +71,24 @@ struct dampr_ctx {
     size_t up_tmp_bytes[2] = {0, 0};
     cudaEvent_t up_tmp_ev[2] = {nullptr, nullptr};
     int up_tmp_next = 0;
+    // page-locked blocks that results are downloaded into (result_lease in ctx.cu); a leased block belongs to the
+    // caller until it is released, whatever the context does meanwhile
+    struct ResultBlock {
+        void *p;
+        size_t bytes;
+        bool leased;
+    };
+    std::vector<ResultBlock> result_blocks;
+    std::mutex result_mu;   // (a lease may be released from another host thread)
 };
+
+// A page-locked block of at least `bytes` from the context's result arena: *lease is its handle for result_release,
+// 0 (and *host_ptr nullptr) when `bytes` is more than the "host_result_cache_bytes" option or page-locked memory has
+// run out: the caller then downloads into pageable memory. Free blocks are reused, new ones are sized in steps of
+// 1.5x, and released blocks are only given back to the system while the arena holds more than the option.
+void result_lease(dampr_ctx *ctx, size_t bytes, void **host_ptr, u64 *lease);
+void result_release(dampr_ctx *ctx, u64 lease);
+extern long long g_result_cache_bytes;
 
 // Host <-> device copies that stay at PCIe speed for pageable host memory: the bytes go through the
 // context's page-locked ring, moved on the host side by several threads, instead of through the driver's

@@ -132,6 +132,7 @@ void pool_trim(dampr_ctx *ctx, size_t keep_bytes) {
 int g_text_ctas = 4;
 int g_file_cufile = 0;         // 1: file ingest through cuFile (GPUDirect Storage) instead of the page-locked ring
 int g_cufile_threads = 8;
+long long g_result_cache_bytes = 64ll << 20;   // page-locked result blocks / sink buffers kept ("host_result_cache_bytes")
 int g_host_threads_cap = 16;   // copy threads per staged transfer (dampr_set_option "host_threads")
 
 // ---- staged transfers ---------------------------------------------------------------------------
@@ -321,6 +322,60 @@ int copy_threads() {
 
 bool host_is_pinned(const void *p) { return is_pinned(p); }
 
+void result_lease(dampr_ctx *ctx, size_t bytes, void **host_ptr, u64 *lease) {
+    *host_ptr = nullptr;
+    *lease = 0;
+    if (bytes == 0 || (long long)bytes > g_result_cache_bytes) return;
+    std::lock_guard<std::mutex> lk(ctx->result_mu);
+    int best = -1;
+    for (int i = 0; i < (int)ctx->result_blocks.size(); ++i) {
+        const auto &b = ctx->result_blocks[i];
+        if (!b.leased && b.bytes >= bytes && (best < 0 || b.bytes < ctx->result_blocks[best].bytes)) best = i;
+    }
+    if (best < 0) {
+        // 1 MB, 1.5 MB, 2 MB, 3 MB, 4 MB ...: a result that grows a little from call to call finds its block again
+        size_t sz = 1u << 20;
+        while (sz < bytes) sz = (sz & (sz - 1)) ? (sz / 3) * 4 : sz + sz / 2;
+        void *p = nullptr;
+        if (cudaHostAlloc(&p, sz, cudaHostAllocDefault) != cudaSuccess) {
+            cudaGetLastError();
+            return;
+        }
+        best = -1;
+        for (int i = 0; i < (int)ctx->result_blocks.size() && best < 0; ++i)
+            if (!ctx->result_blocks[i].p) best = i;
+        if (best < 0) {
+            ctx->result_blocks.push_back({nullptr, 0, false});
+            best = (int)ctx->result_blocks.size() - 1;
+        }
+        ctx->result_blocks[best].p = p;
+        ctx->result_blocks[best].bytes = sz;
+    }
+    ctx->result_blocks[best].leased = true;
+    *host_ptr = ctx->result_blocks[best].p;
+    *lease = (u64)best + 1;
+}
+
+void result_release(dampr_ctx *ctx, u64 lease) {
+    std::lock_guard<std::mutex> lk(ctx->result_mu);
+    if (lease == 0 || lease > ctx->result_blocks.size() || !ctx->result_blocks[lease - 1].leased) return;
+    ctx->result_blocks[lease - 1].leased = false;
+    size_t total = 0;
+    for (const auto &b : ctx->result_blocks) total += b.p ? b.bytes : 0;
+    // above the bound the largest free blocks go back to the system (their slots stay: handles are indices)
+    while ((long long)total > g_result_cache_bytes) {
+        int big = -1;
+        for (int i = 0; i < (int)ctx->result_blocks.size(); ++i) {
+            const auto &b = ctx->result_blocks[i];
+            if (b.p && !b.leased && (big < 0 || b.bytes > ctx->result_blocks[big].bytes)) big = i;
+        }
+        if (big < 0) break;
+        cudaFreeHost(ctx->result_blocks[big].p);
+        total -= ctx->result_blocks[big].bytes;
+        ctx->result_blocks[big] = {nullptr, 0, false};
+    }
+}
+
 int staged_h2d(dampr_ctx *ctx, void *dst, const void *src, size_t bytes, cudaStream_t st) {
     if (bytes == 0) return DAMPR_OK;
     if (bytes < (8u << 20) || is_pinned(src)) {
@@ -494,6 +549,9 @@ int32_t dampr_ctx_destroy(dampr_ctx *ctx) {
         if (ctx->dstage_slot[i]) cudaFreeHost(ctx->dstage_slot[i]);
         if (ctx->dstage_ev[i]) cudaEventDestroy(ctx->dstage_ev[i]);
     }
+    // (a block somebody still holds a lease on is theirs: it is left allocated)
+    for (auto &b : ctx->result_blocks)
+        if (b.p && !b.leased) cudaFreeHost(b.p);
     cudaStreamDestroy(ctx->stream);
     cudaStreamDestroy(ctx->copy);
     delete ctx;
@@ -511,6 +569,21 @@ int32_t dampr_ctx_sync(dampr_ctx *ctx) {
 int32_t dampr_ctx_sync_copy(dampr_ctx *ctx) {
     if (!ctx) return DAMPR_ERR_ARG;
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->copy));
+    return DAMPR_OK;
+}
+
+int32_t dampr_result_lease(dampr_ctx *ctx, uint64_t bytes, void **host_ptr, uint64_t *lease) {
+    ARG_CHECK(ctx, ctx && host_ptr && lease, "null");
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    u64 id = 0;
+    result_lease(ctx, bytes, host_ptr, &id);
+    *lease = id;
+    return DAMPR_OK;
+}
+
+int32_t dampr_result_release(dampr_ctx *ctx, uint64_t lease) {
+    if (!ctx) return DAMPR_ERR_ARG;
+    result_release(ctx, lease);
     return DAMPR_OK;
 }
 

@@ -975,6 +975,11 @@ int32_t dampr_set_option(const char *name, int64_t value) {
         g_host_threads_cap = (int)value;
         return DAMPR_OK;
     }
+    if (!strcmp(name, "host_result_cache_bytes")) {
+        if (value < 0) return DAMPR_ERR_ARG;
+        g_result_cache_bytes = value;
+        return DAMPR_OK;
+    }
     if (!strcmp(name, "text_kernel")) {
         if (value != 1 && value != 2) return DAMPR_ERR_ARG;
         g_text_kernel = (int)value;

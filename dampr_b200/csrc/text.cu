@@ -23,6 +23,10 @@
 #include <thread>
 
 #include <charconv>
+#include <chrono>
+#include <condition_variable>
+#include <memory>
+#include <mutex>
 #include <cmath>
 #include <limits>
 
@@ -879,18 +883,9 @@ __global__ void table_words_kernel(const u64 *__restrict__ keys, const u64 *__re
 
 }  // namespace
 
-extern "C" int32_t dampr_table_fetch_words(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, int32_t mode,
-                                           uint32_t width, uint8_t *words, uint64_t *counts, uint64_t *codes,
-                                           uint64_t *reps, uint64_t cap, uint64_t *n) {
-    ARG_CHECK(ctx, ctx && t && n, "null");
-    ARG_CHECK(ctx, width >= 16 && width <= 256 && (width % 8) == 0, "width must be a multiple of 8 in [16, 256]");
-    uint64_t st[8];
-    int rc = dampr_table_stats(ctx, t, st);
-    if (rc) return rc;
-    *n = st[0];
-    if (!words) return DAMPR_OK;
-    ARG_CHECK(ctx, cap >= st[0] && counts, "fetch arrays too small");   // codes / reps are optional
-    u64 m = st[0];
+// the m entries of the table, decoded, into host arrays (page-locked ones are copied into directly)
+static int fetch_words_into(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, int32_t mode, uint32_t width, u64 m,
+                            uint8_t *words, uint64_t *counts, uint64_t *codes, uint64_t *reps) {
     t->ext_n = 0;
     if (m == 0) return DAMPR_OK;
     // the count column stays on the device (t->ext) for dampr_count_dictionary
@@ -933,6 +928,48 @@ extern "C" int32_t dampr_table_fetch_words(dampr_ctx *ctx, dampr_table *t, dampr
     }
     if (rc2 == DAMPR_OK) t->ext_n = m;
     return rc2;
+}
+
+extern "C" int32_t dampr_table_fetch_words(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, int32_t mode,
+                                           uint32_t width, uint8_t *words, uint64_t *counts, uint64_t *codes,
+                                           uint64_t *reps, uint64_t cap, uint64_t *n) {
+    ARG_CHECK(ctx, ctx && t && n, "null");
+    ARG_CHECK(ctx, width >= 16 && width <= 256 && (width % 8) == 0, "width must be a multiple of 8 in [16, 256]");
+    uint64_t st[8];
+    int rc = dampr_table_stats(ctx, t, st);
+    if (rc) return rc;
+    *n = st[0];
+    if (!words) return DAMPR_OK;
+    ARG_CHECK(ctx, cap >= st[0] && counts, "fetch arrays too small");   // codes / reps are optional
+    return fetch_words_into(ctx, t, tb, mode, width, st[0], words, counts, codes, reps);
+}
+
+extern "C" int32_t dampr_table_fetch_words_leased(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, int32_t mode,
+                                                  uint32_t width, int32_t with_codes, void **host_ptr,
+                                                  uint64_t *lease, uint64_t *n) {
+    ARG_CHECK(ctx, ctx && t && n && host_ptr && lease, "null");
+    ARG_CHECK(ctx, width >= 16 && width <= 256 && (width % 8) == 0, "width must be a multiple of 8 in [16, 256]");
+    *host_ptr = nullptr;
+    *lease = 0;
+    uint64_t st[8];
+    int rc = dampr_table_stats(ctx, t, st);
+    if (rc) return rc;
+    const u64 m = *n = st[0];
+    if (m == 0) return DAMPR_OK;
+    u64 id = 0;
+    result_lease(ctx, m * (width + (with_codes ? 24 : 8)), host_ptr, &id);
+    if (!id) return DAMPR_OK;
+    u8 *words = (u8 *)*host_ptr;
+    uint64_t *counts = (uint64_t *)(words + m * width);
+    rc = fetch_words_into(ctx, t, tb, mode, width, m, words, counts, with_codes ? counts + m : nullptr,
+                          with_codes ? counts + 2 * m : nullptr);
+    if (rc) {
+        result_release(ctx, id);
+        *host_ptr = nullptr;
+        return rc;
+    }
+    *lease = id;
+    return DAMPR_OK;
 }
 
 extern "C" int32_t dampr_table_extracted_counts(dampr_ctx *ctx, dampr_table *t, uint64_t *dev_ptr, uint64_t *n) {
@@ -1058,10 +1095,11 @@ __global__ void dict_big_kernel(const ulonglong2 *__restrict__ big, u64 nbig, co
 
 }  // namespace
 
-extern "C" int32_t dampr_count_dictionary(dampr_ctx *ctx, const uint64_t *counts, uint64_t n, uint32_t stride,
-                                          const int64_t *extra, uint32_t n_extra, int64_t *uniq, uint32_t *inv,
-                                          uint32_t *rows, uint64_t *n_uniq) {
-    ARG_CHECK(ctx, ctx && uniq && inv && rows && n_uniq && stride >= 1, "null");
+// host_ptr != nullptr: the outputs go into one lease of the context's result arena, taken once the number of distinct
+// values is known (uniq, inv and rows are then ignored); *lease stays 0 when the arena gives none
+static int count_dictionary(dampr_ctx *ctx, const uint64_t *counts, uint64_t n, uint32_t stride, const int64_t *extra,
+                            uint32_t n_extra, int64_t *uniq, uint32_t *inv, uint32_t *rows, uint64_t *n_uniq,
+                            void **host_ptr, uint64_t *lease) {
     ARG_CHECK(ctx, (counts || n == 0) && (extra || n_extra == 0), "null column");
     const u64 N = n + n_extra;
     ARG_CHECK(ctx, N < (1ULL << 32), "more than 2^32 rows");
@@ -1147,12 +1185,42 @@ extern "C" int32_t dampr_count_dictionary(dampr_ctx *ctx, const uint64_t *counts
         if (red) dampr_kv_destroy(ctx, red);
         if (rc) return rc;
     }
-    CUDA_TRY(ctx, cudaMemcpyAsync(inv, d_inv, N * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(ctx, cudaMemcpyAsync(uniq, d_uniq, m * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(ctx, cudaMemcpyAsync(rows, d_rows, m * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     *n_uniq = m;
+    u64 id = 0;
+    if (host_ptr) {
+        // uniq[m] | inv[N] | rows[m]
+        result_lease(ctx, m * 8 + N * 4 + m * 4, host_ptr, &id);
+        if (!id) return DAMPR_OK;
+        uniq = (int64_t *)*host_ptr;
+        inv = (uint32_t *)(uniq + m);
+        rows = inv + N;
+    }
+    cudaError_t e = cudaMemcpyAsync(inv, d_inv, N * 4, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(uniq, d_uniq, m * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(rows, d_rows, m * 4, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) {
+        if (id) result_release(ctx, id);
+        return set_err(ctx, DAMPR_ERR_CUDA, "count dictionary download failed: %s", cudaGetErrorString(e));
+    }
+    if (host_ptr) *lease = id;
     return DAMPR_OK;
+}
+
+extern "C" int32_t dampr_count_dictionary(dampr_ctx *ctx, const uint64_t *counts, uint64_t n, uint32_t stride,
+                                          const int64_t *extra, uint32_t n_extra, int64_t *uniq, uint32_t *inv,
+                                          uint32_t *rows, uint64_t *n_uniq) {
+    ARG_CHECK(ctx, ctx && uniq && inv && rows && n_uniq && stride >= 1, "null");
+    return count_dictionary(ctx, counts, n, stride, extra, n_extra, uniq, inv, rows, n_uniq, nullptr, nullptr);
+}
+
+extern "C" int32_t dampr_count_dictionary_leased(dampr_ctx *ctx, const uint64_t *counts, uint64_t n, uint32_t stride,
+                                                 const int64_t *extra, uint32_t n_extra, void **host_ptr,
+                                                 uint64_t *lease, uint64_t *n_uniq) {
+    ARG_CHECK(ctx, ctx && host_ptr && lease && n_uniq && stride >= 1, "null");
+    *host_ptr = nullptr;
+    *lease = 0;
+    return count_dictionary(ctx, counts, n, stride, extra, n_extra, nullptr, nullptr, nullptr, n_uniq, host_ptr, lease);
 }
 
 // ---- host-side sink formatting (SinkWriter, dataset.py:264-282: one print(value) per record) --------
@@ -1162,6 +1230,120 @@ extern "C" int32_t dampr_count_dictionary(dampr_ctx *ctx, const uint64_t *counts
 //   2  dictionary of int64 values    ptr = u32 inv[n], aux = int64 values[m], widths = m (decimal text)
 // out == NULL: only *out_len is computed.
 namespace {
+// Process-wide pool of host workers for the sink, the row joiner and dampr_host_unique_small: created on first use,
+// parked on a condition variable between calls and joined when the library is unloaded or the process exits. A call
+// holds lock() for as long as it uses the pool or its buffers; run(T, fn) calls fn(0) .. fn(T - 1), the caller taking
+// its share, and returns when all have finished. A job is its own heap object, so a worker that wakes late sees a
+// finished job and nothing of the caller's frame.
+class HostPool {
+    struct Job {
+        const std::function<void(int)> *fn;
+        int T;
+        std::atomic<int> next{0}, left{0};
+    };
+
+  public:
+    static constexpr int MAX_TASKS = 16;
+    static HostPool &get() {
+        static HostPool p;
+        return p;
+    }
+    static int width() { return (int)std::max(1u, std::min(std::thread::hardware_concurrency(), (unsigned)MAX_TASKS)); }
+    std::unique_lock<std::mutex> lock() { return std::unique_lock<std::mutex>(job_mu_); }
+    void run(int T, const std::function<void(int)> &fn) {
+        if (T <= 1) {
+            if (T == 1) fn(0);
+            return;
+        }
+        auto job = std::make_shared<Job>();
+        job->fn = &fn;
+        job->T = T;
+        job->left.store(T);
+        {
+            std::lock_guard<std::mutex> lk(mu_);
+            if (pid_ != getpid()) {
+                // a forked child has none of its parent's threads: their handles are abandoned, not joined
+                workers_ = new std::vector<std::thread>();
+                pid_ = getpid();
+            }
+            while ((int)workers_->size() < std::min(T, width()) - 1) {
+                workers_->emplace_back([this] { loop(); });
+                ++started_;
+            }
+            cur_ = job;
+            ++gen_;
+        }
+        cv_.notify_all();
+        work(*job);
+        std::unique_lock<std::mutex> lk(mu_);
+        done_cv_.wait(lk, [&] { return job->left.load() == 0; });
+    }
+    // task t's output buffer of at least `bytes`, kept between calls so that its pages stay mapped; nullptr when
+    // `bytes` is more than a task's share of the "host_result_cache_bytes" option (the caller then uses malloc)
+    u8 *buffer(int t, size_t bytes) {
+        if (t >= MAX_TASKS || bytes > (size_t)g_result_cache_bytes / MAX_TASKS) return nullptr;
+        if (cap_[t] < bytes) {
+            free(buf_[t]);
+            buf_[t] = (u8 *)malloc(bytes);
+            cap_[t] = buf_[t] ? bytes : 0;
+        }
+        return buf_[t];
+    }
+    u64 threads_started() {
+        std::lock_guard<std::mutex> lk(mu_);
+        return started_;
+    }
+
+  private:
+    HostPool() : workers_(new std::vector<std::thread>()), pid_(getpid()) {}
+    ~HostPool() {
+        {
+            std::lock_guard<std::mutex> lk(mu_);
+            stop_ = true;
+        }
+        cv_.notify_all();
+        if (pid_ == getpid()) {
+            for (auto &t : *workers_) t.join();
+            delete workers_;
+        }
+        for (u8 *b : buf_) free(b);
+    }
+    void work(Job &j) {
+        for (;;) {
+            const int t = j.next.fetch_add(1);
+            if (t >= j.T) break;
+            (*j.fn)(t);
+            if (j.left.fetch_sub(1) == 1) {
+                std::lock_guard<std::mutex> lk(mu_);
+                done_cv_.notify_all();
+            }
+        }
+    }
+    void loop() {
+        u64 seen = 0;
+        for (;;) {
+            std::shared_ptr<Job> job;
+            {
+                std::unique_lock<std::mutex> lk(mu_);
+                cv_.wait(lk, [&] { return stop_ || gen_ != seen; });
+                if (stop_) return;
+                seen = gen_;
+                job = cur_;
+            }
+            work(*job);
+        }
+    }
+    std::mutex job_mu_, mu_;
+    std::condition_variable cv_, done_cv_;
+    std::vector<std::thread> *workers_;
+    pid_t pid_;
+    std::shared_ptr<Job> cur_;
+    u64 gen_ = 0, started_ = 0;
+    bool stop_ = false;
+    u8 *buf_[MAX_TASKS] = {};
+    size_t cap_[MAX_TASKS] = {};
+};
+
 struct JoinArgs {
     u64 n;
     int ncols;
@@ -1179,6 +1361,7 @@ struct IntDicts {
     std::vector<std::vector<u32>> offs;
     std::vector<int32_t> kinds;
     std::vector<const void *> aux, aux2;
+    std::vector<u32> longest;   // per column: the longest string of a dictionary built here (0 otherwise)
 };
 // repr(float) of CPython (float_repr_style 'short': PyOS_double_to_string(x, 'r', 0, Py_DTSF_ADD_DOT_0), i.e. the
 // shortest digit string that round-trips, laid out in fixed notation when -4 < decpt <= 16 and with an exponent of
@@ -1264,8 +1447,10 @@ static int format_py_float(double v, char *out) {
     return n;
 }
 
-static void lower_int_dicts(int ncols, const int32_t *kinds, const uint32_t *widths, const void *const *aux,
-                            const void *const *aux2, IntDicts &d) {
+// (the caller holds the pool's lock)
+static void lower_int_dicts(HostPool &pool, int ncols, const int32_t *kinds, const uint32_t *widths,
+                            const void *const *aux, const void *const *aux2, IntDicts &d) {
+    d.longest.assign(ncols, 0);
     d.kinds.assign(kinds, kinds + ncols);
     d.aux.assign(aux, aux + ncols);
     d.aux2.assign(aux2, aux2 + ncols);
@@ -1274,28 +1459,24 @@ static void lower_int_dicts(int ncols, const int32_t *kinds, const uint32_t *wid
     for (int c = 0; c < ncols; ++c) {
         if (kinds[c] == 3) {
             // dictionary of float64 values: ptr = u32 inv[n], aux = double values[m], widths = m -> kind 1 with
-            // Python's repr of every distinct value, formatted here (a few threads for large dictionaries)
+            // Python's repr of every distinct value, formatted here (on the pool for large dictionaries)
             const double *vals = (const double *)aux[c];
             const u32 m = widths[c];
             auto &blob = d.blobs[c];
             auto &off = d.offs[c];
             std::vector<char> slots((size_t)m * 24 + 24);
             std::vector<u8> lens((size_t)m + 1);
-            const unsigned hw = std::thread::hardware_concurrency();
-            const int T = (int)std::max<u32>(1, std::min<u32>(std::min(hw, 8u), m / 4096));
-            auto work = [&](int t) {
+            const int T = (int)std::max<u32>(1, std::min<u32>(HostPool::width(), m / 1024));
+            pool.run(T, [&](int t) {
                 const u32 lo = (u32)((u64)m * t / T), hi = (u32)((u64)m * (t + 1) / T);
                 for (u32 j = lo; j < hi; ++j) lens[j] = (u8)format_py_float(vals[j], slots.data() + (size_t)j * 24);
-            };
-            {
-                std::vector<std::thread> th;
-                for (int t = 1; t < T; ++t) th.emplace_back(work, t);
-                work(0);
-                for (auto &x : th) x.join();
-            }
+            });
             off.resize((size_t)m + 1);
             off[0] = 0;
-            for (u32 j = 0; j < m; ++j) off[j + 1] = off[j] + lens[j];
+            for (u32 j = 0; j < m; ++j) {
+                off[j + 1] = off[j] + lens[j];
+                d.longest[c] = std::max<u32>(d.longest[c], lens[j]);
+            }
             blob.resize((size_t)off[m] + 1);
             for (u32 j = 0; j < m; ++j) memcpy(blob.data() + off[j], slots.data() + (size_t)j * 24, lens[j]);
             d.kinds[c] = 1;
@@ -1323,6 +1504,7 @@ static void lower_int_dicts(int ncols, const int32_t *kinds, const uint32_t *wid
             if (v < 0) tmp[--k] = '-';
             blob.insert(blob.end(), tmp + k, tmp + 24);
             off[j + 1] = (u32)blob.size();
+            d.longest[c] = std::max<u32>(d.longest[c], (u32)(24 - k));
         }
         if (blob.empty()) blob.push_back(0);
         d.kinds[c] = 1;
@@ -1443,31 +1625,48 @@ extern "C" int32_t dampr_host_join_tsv(uint64_t n, int32_t ncols, const int32_t 
                                        const uint32_t *widths, const void *const *aux, const void *const *aux2,
                                        uint8_t *out, uint64_t cap, uint64_t *out_len) {
     if (!kinds || !ptrs || !out_len || ncols < 1 || ncols > 16) return DAMPR_ERR_ARG;
+    HostPool &pool = HostPool::get();
+    auto pool_lock = pool.lock();
     IntDicts idc;
-    lower_int_dicts(ncols, kinds, widths, aux, aux2, idc);
+    lower_int_dicts(pool, ncols, kinds, widths, aux, aux2, idc);
     JoinArgs a{n, ncols, idc.kinds.data(), ptrs, widths, idc.aux.data(), idc.aux2.data()};
-    unsigned hw = std::thread::hardware_concurrency();
-    int T = (int)std::min<u64>(std::max(1u, std::min(hw, 16u)), std::max<u64>(1, n / 16384));
+    const int T = (int)std::min<u64>(HostPool::width(), std::max<u64>(1, n / 16384));
     std::vector<u64> lens(T, 0), offs(T + 1, 0);
-    auto span = [&](int t) { return std::make_pair(n * t / T, n * (t + 1) / T); };
-    {
-        std::vector<std::thread> th;
-        for (int t = 1; t < T; ++t) th.emplace_back([&, t] { auto r = span(t); lens[t] = join_rows(a, r.first, r.second, nullptr); });
-        auto r0 = span(0);
-        lens[0] = join_rows(a, r0.first, r0.second, nullptr);
-        for (auto &x : th) x.join();
-    }
+    pool.run(T, [&](int t) { lens[t] = join_rows(a, n * t / T, n * (t + 1) / T, nullptr); });
     for (int t = 0; t < T; ++t) offs[t + 1] = offs[t] + lens[t];
     *out_len = offs[T];
     if (!out) return DAMPR_OK;
     if (offs[T] > cap) return DAMPR_ERR_ARG;
-    {
-        std::vector<std::thread> th;
-        for (int t = 1; t < T; ++t) th.emplace_back([&, t] { auto r = span(t); join_rows(a, r.first, r.second, out + offs[t]); });
-        auto r0 = span(0);
-        join_rows(a, r0.first, r0.second, out);
-        for (auto &x : th) x.join();
-    }
+    pool.run(T, [&](int t) { join_rows(a, n * t / T, n * (t + 1) / T, out + offs[t]); });
+    return DAMPR_OK;
+}
+
+// Host-clock split of the last sink_rows call, in milliseconds: the calling thread's dictionary preparation, then the
+// largest value any worker saw for the delay before it started, open(), row formatting, write() and close().
+namespace {
+struct SinkTimes {
+    double prep = 0, start = 0, open = 0, format = 0, write = 0, close = 0;
+};
+std::mutex g_sink_times_mu;
+SinkTimes g_sink_times;
+using SinkClock = std::chrono::steady_clock;
+inline double ms_since(SinkClock::time_point t0) {
+    return std::chrono::duration<double, std::milli>(SinkClock::now() - t0).count();
+}
+}  // namespace
+
+extern "C" int32_t dampr_host_sink_timings(double *out_ms) {
+    if (!out_ms) return DAMPR_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g_sink_times_mu);
+    const SinkTimes &s = g_sink_times;
+    const double v[6] = {s.prep, s.start, s.open, s.format, s.write, s.close};
+    memcpy(out_ms, v, sizeof v);
+    return DAMPR_OK;
+}
+
+extern "C" int32_t dampr_host_pool_threads(uint64_t *started) {
+    if (!started) return DAMPR_ERR_ARG;
+    *started = HostPool::get().threads_started();
     return DAMPR_OK;
 }
 
@@ -1481,51 +1680,76 @@ static int32_t sink_rows(const char *prefix, uint32_t first_index, uint32_t max_
                          uint64_t *out_len, uint32_t *n_files, const RowFmt *fmt) {
     if (!prefix || !kinds || !ptrs || !out_len || !n_files || ncols < 1 || ncols > 16 || max_files < 1)
         return DAMPR_ERR_ARG;
+    const auto t_call = SinkClock::now();
+    HostPool &pool = HostPool::get();
+    auto pool_lock = pool.lock();
     IntDicts idc;
-    lower_int_dicts(ncols, kinds, widths, aux, aux2, idc);
+    lower_int_dicts(pool, ncols, kinds, widths, aux, aux2, idc);
     kinds = idc.kinds.data();
     aux = idc.aux.data();
     aux2 = idc.aux2.data();
     JoinArgs a{n, ncols, kinds, ptrs, widths, aux, aux2};
-    // longest possible row: fixed widths + the longest string of every dictionary + separators
-    u64 max_row = (u64)ncols;
+    // the fixed part of the longest possible row: fixed widths, the longest string of every dictionary formatted
+    // above, separators. A caller's own dictionary gives no length: each writer bounds it over its own rows.
+    u64 row_fixed = (u64)ncols;
     if (fmt) {
-        max_row = fmt->row_end.size();
-        for (auto &x : fmt->pre) max_row += x.size();
+        row_fixed = fmt->row_end.size();
+        for (auto &x : fmt->pre) row_fixed += x.size();
     }
-    for (int c = 0; c < ncols; ++c) {
-        if (kinds[c] == 0) {
-            max_row += widths[c];
-        } else {
+    for (int c = 0; c < ncols; ++c) row_fixed += kinds[c] == 0 ? widths[c] : idc.longest[c];
+    const int T = (int)std::min<u64>(std::min<u64>(HostPool::width(), max_files), std::max<u64>(1, n / 32768));
+    std::vector<u64> lens(T, 0);
+    std::vector<SinkTimes> tms(T);
+    tms[0].prep = ms_since(t_call);
+    const auto t_go = SinkClock::now();
+    std::atomic<int> bad{0};
+    pool.run(T, [&](int t) {
+        SinkTimes &tm = tms[t];
+        tm.start = ms_since(t_go);
+        auto t0 = SinkClock::now();
+        const u64 lo = n * t / T, hi = n * (t + 1) / T;
+        u64 max_row = row_fixed;
+        for (int c = 0; c < ncols; ++c) {
+            if (kinds[c] == 0 || idc.blobs[c].size()) continue;
             const u32 *off = (const u32 *)aux2[c];
             const u32 *inv = (const u32 *)ptrs[c];
             u32 m = 0;
-            for (u64 i = 0; i < n; ++i) m = std::max(m, inv[i]);
+            for (u64 i = lo; i < hi; ++i) m = std::max(m, inv[i]);
             u32 longest = 0;
             for (u32 j = 0; j <= m; ++j) longest = std::max(longest, off[j + 1] - off[j]);
             max_row += longest;
         }
-    }
-    unsigned hw = std::thread::hardware_concurrency();
-    const int T = (int)std::min<u64>(std::min<u64>(std::max(1u, std::min(hw, 16u)), max_files), std::max<u64>(1, n / 32768));
-    std::vector<u64> lens(T, 0);
-    std::atomic<int> bad{0};
-    auto work = [&](int t) {
-        const u64 lo = n * t / T, hi = n * (t + 1) / T;
-        std::string path = std::string(prefix) + std::to_string(first_index + (u32)t);
-        int fd = open(path.c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0644);
-        if (fd < 0) {
-            bad.store(1);
-            return;
-        }
-        // malloc of the upper bound: pages that are never written cost nothing, one pass over the rows
-        u8 *buf = (hi > lo) ? (u8 *)malloc((hi - lo) * max_row + 64) : nullptr;
+        // the upper bound of the range: pages that are never written cost nothing, one pass over the rows
+        const size_t need = (hi - lo) * max_row + 64;
+        u8 *buf = hi > lo ? pool.buffer(t, need) : nullptr;
+        const bool own = hi > lo && !buf;
+        if (own) buf = (u8 *)malloc(need);
         if (hi > lo && !buf) {
             bad.store(1);
-            close(fd);
             return;
         }
-        const u64 len = (hi > lo) ? (fmt ? join_rows_fmt(a, *fmt, lo, hi, buf) : join_rows_fast(a, lo, hi, buf)) : 0;
+        // Creating files in one directory serialises on the directory's lock: 16 writers that open at the same
+        // moment queue for about 2 ms. Writer t opens its file after the first t/T of its rows, so the creations are
+        // spread over the formatting and none waits for another.
+        auto rows = [&](u64 from, u64 to, u8 *out) {
+            return to > from ? (fmt ? join_rows_fmt(a, *fmt, from, to, out) : join_rows_fast(a, from, to, out)) : 0;
+        };
+        const u64 mid = lo + (hi - lo) * (u64)t / (u64)T;
+        u64 len = rows(lo, mid, buf);
+        tm.format = ms_since(t0);
+        t0 = SinkClock::now();
+        std::string path = std::string(prefix) + std::to_string(first_index + (u32)t);
+        int fd = open(path.c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0644);
+        tm.open = ms_since(t0);
+        if (fd < 0) {
+            bad.store(1);
+            if (own) free(buf);
+            return;
+        }
+        t0 = SinkClock::now();
+        len += rows(mid, hi, buf + len);
+        tm.format += ms_since(t0);
+        t0 = SinkClock::now();
         u64 done = 0;
         while (done < len) {
             ssize_t w = write(fd, buf + done, len - done);
@@ -1535,15 +1759,25 @@ static int32_t sink_rows(const char *prefix, uint32_t first_index, uint32_t max_
             }
             done += (u64)w;
         }
-        free(buf);
+        tm.write = ms_since(t0);
+        t0 = SinkClock::now();
+        if (own) free(buf);
         if (close(fd) != 0) bad.store(1);
+        tm.close = ms_since(t0);
         lens[t] = len;
-    };
+    });
     {
-        std::vector<std::thread> th;
-        for (int t = 1; t < T; ++t) th.emplace_back(work, t);
-        work(0);
-        for (auto &x : th) x.join();
+        SinkTimes mx;
+        mx.prep = tms[0].prep;
+        for (const SinkTimes &x : tms) {
+            mx.start = std::max(mx.start, x.start);
+            mx.open = std::max(mx.open, x.open);
+            mx.format = std::max(mx.format, x.format);
+            mx.write = std::max(mx.write, x.write);
+            mx.close = std::max(mx.close, x.close);
+        }
+        std::lock_guard<std::mutex> lk(g_sink_times_mu);
+        g_sink_times = mx;
     }
     u64 total = 0;
     for (int t = 0; t < T; ++t) total += lens[t];
@@ -1591,8 +1825,9 @@ extern "C" int32_t dampr_host_unique_small(const int64_t *col, uint64_t n, uint6
     // (3) look every row's rank up
     std::vector<u32> rank(table, 0);
     std::vector<u32> first(first_row ? table : 0, 0xFFFFFFFFu);
-    const unsigned hw = std::thread::hardware_concurrency();
-    const int T = (int)std::max<u64>(1, std::min<u64>(std::min(hw, 8u), n / 65536));
+    HostPool &pool = HostPool::get();
+    auto pool_lock = pool.lock();
+    const int T = (int)std::max<u64>(1, std::min<u64>(std::min(HostPool::width(), 8), n / 65536));
     std::vector<std::vector<std::pair<int64_t, u64>>> bigs((size_t)T);
     auto mark = [&](int t) {
         const u64 lo = n * t / T, hi = n * (t + 1) / T;
@@ -1612,12 +1847,7 @@ extern "C" int32_t dampr_host_unique_small(const int64_t *col, uint64_t n, uint6
             }
         }
     };
-    {
-        std::vector<std::thread> th;
-        for (int t = 1; t < T; ++t) th.emplace_back(mark, t);
-        mark(0);
-        for (auto &x : th) x.join();
-    }
+    pool.run(T, mark);
     u64 nb = 0;
     for (auto &big : bigs) {
         if (nb + big.size() > big_cap) return DAMPR_ERR_ARG;
@@ -1642,12 +1872,7 @@ extern "C" int32_t dampr_host_unique_small(const int64_t *col, uint64_t n, uint6
             if (v >= 0 && (u64)v < table) inv[i] = rank[(u64)v];
         }
     };
-    {
-        std::vector<std::thread> th;
-        for (int t = 1; t < T; ++t) th.emplace_back(look, t);
-        look(0);
-        for (auto &x : th) x.join();
-    }
+    pool.run(T, look);
     *n_uniq = m;
     *n_big = nb;
     return DAMPR_OK;

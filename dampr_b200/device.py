@@ -163,8 +163,13 @@ def load_library():
     _sig(lib, "dampr_table_fetch", vp, vp, vp, vp, vp, u64, pu64)
     _sig(lib, "dampr_table_to_kv", vp, vp, pvp)
     _sig(lib, "dampr_table_fetch_words", vp, vp, vp, i32, u32, vp, vp, vp, vp, u64, pu64)
+    _sig(lib, "dampr_table_fetch_words_leased", vp, vp, vp, i32, u32, i32, pvp, pu64, pu64)
     _sig(lib, "dampr_table_extracted_counts", vp, vp, pu64, pu64)
     _sig(lib, "dampr_count_dictionary", vp, vp, u64, u32, vp, u32, vp, vp, vp, pu64)
+    _sig(lib, "dampr_count_dictionary_leased", vp, vp, u64, u32, vp, u32, pvp, pu64, pu64)
+    _sig(lib, "dampr_result_lease", vp, u64, pvp, pu64)
+    _sig(lib, "dampr_result_release", vp, u64)
+    _sig(lib, "dampr_host_pool_threads", pu64)
     _sig(lib, "dampr_host_eval_f64", vp, u64, vp, u32, vp, vp, vp)
     _sig(lib, "dampr_kv_decode_words", vp, vp, i32, u32, vp)
     _sig(lib, "dampr_host_join_tsv", u64, i32, vp, vp, vp, vp, vp, vp, u64, pu64)
@@ -172,6 +177,7 @@ def load_library():
          C.POINTER(C.c_uint32))
     _sig(lib, "dampr_host_sink_fmt", C.c_char_p, C.c_uint32, C.c_uint32, u64, i32, vp, vp, vp, vp, vp, vp, C.c_char_p, pu64,
          C.POINTER(C.c_uint32))
+    _sig(lib, "dampr_host_sink_timings", C.POINTER(C.c_double))
     _sig(lib, "dampr_host_unique_small", vp, u64, u64, vp, pu64, vp, vp, vp, vp, u64, pu64)
     _sig(lib, "dampr_kv_create", vp, u64, pvp)
     _sig(lib, "dampr_kv_destroy", vp, vp)
@@ -215,6 +221,12 @@ def set_option(name, value):
         raise DeviceError("unknown option %r" % name)
 
 
+def _apply_result_cache():
+    """settings.host_result_cache_bytes -> the library (read at every call that leases or keeps host memory)"""
+    from . import settings
+    set_option("host_result_cache_bytes", max(0, int(settings.host_result_cache_bytes or 0)))
+
+
 def _ptr(a):
     """Host pointer of a C-contiguous numpy array (or None)."""
     if a is None:
@@ -249,6 +261,31 @@ class PinnedBuffer(object):
     def __del__(self):
         try:
             self.free()
+        except Exception:
+            pass
+
+
+class ResultLease(object):
+    """A page-locked block of a context's result arena (dampr_result_lease) as the base object of numpy arrays:
+    array() returns views whose memory is this block, every view and every slice of one keeps the lease alive, and
+    the block goes back to the arena when the last of them is gone."""
+
+    def __init__(self, ctx, handle, ptr, nbytes):
+        self.ctx, self.handle, self.nbytes = ctx, int(handle), int(nbytes)
+        self.__array_interface__ = {"shape": (self.nbytes,), "typestr": "|u1", "data": (int(ptr), False), "version": 3}
+
+    def array(self, offset, count, dtype):
+        """`count` items of `dtype` at byte `offset` of the block"""
+        dtype = np.dtype(dtype)
+        raw = np.asarray(self)
+        assert raw.base is self and offset + count * dtype.itemsize <= self.nbytes
+        return raw[offset:offset + count * dtype.itemsize].view(dtype)
+
+    def __del__(self):
+        try:
+            if self.handle and self.ctx.h is not None:
+                self.ctx.lib.dampr_result_release(self.ctx.h, self.handle)
+            self.handle = 0
         except Exception:
             pass
 
@@ -430,11 +467,25 @@ class Ctx(object):
         `stride`-th), then the host values `extra`. None when a value is negative."""
         ex = np.ascontiguousarray(extra, dtype=np.int64)
         N = int(n) + len(ex)
+        cptr = C.c_void_p(int(dev_ptr)) if n else None
+        _apply_result_cache()
+        # into one page-locked block of the result arena; without one (see dampr_result_lease), into pageable arrays
+        m, p, lease = C.c_uint64(0), C.c_void_p(), C.c_uint64(0)
+        rc = self.lib.dampr_count_dictionary_leased(self.h, cptr, int(n), int(stride), _ptr(ex) if len(ex) else None,
+                                                    len(ex), C.byref(p), C.byref(lease), C.byref(m))
+        if rc == -5:   # DAMPR_ERR_UNSUPPORTED
+            return None
+        self.check(rc)
+        if lease.value:
+            m = m.value
+            blk = ResultLease(self, lease.value, p.value, 12 * m + 4 * N)
+            return blk.array(0, m, np.int64), blk.array(8 * m, N, np.uint32), \
+                blk.array(8 * m + 4 * N, m, np.uint32).astype(np.int64)
         uniq = np.empty(max(1, N), dtype=np.int64)
         inv = np.empty(N, dtype=np.uint32)
         rows = np.empty(max(1, N), dtype=np.uint32)
         m = C.c_uint64(0)
-        rc = self.lib.dampr_count_dictionary(self.h, C.c_void_p(int(dev_ptr)) if n else None, int(n), int(stride),
+        rc = self.lib.dampr_count_dictionary(self.h, cptr, int(n), int(stride),
                                              _ptr(ex) if len(ex) else None, len(ex), _ptr(uniq), _ptr(inv),
                                              _ptr(rows), C.byref(m))
         if rc == -5:   # DAMPR_ERR_UNSUPPORTED
@@ -592,6 +643,21 @@ class Table(object):
         when with_codes is false (tables without hashed tokens need neither)."""
         self.fetches += 1
         n = C.c_uint64(0)
+        # one call into one page-locked block of the result arena: the arrays returned are views of it and keep it
+        # leased for as long as any of them lives. Without a block (see dampr_result_lease): pageable arrays, below.
+        p, lease = C.c_void_p(), C.c_uint64(0)
+        _apply_result_cache()
+        self.ctx.check(self.ctx.lib.dampr_table_fetch_words_leased(
+            self.ctx.h, self.h, tb.h if tb is not None else None, int(mode), int(width), 1 if with_codes else 0,
+            C.byref(p), C.byref(lease), C.byref(n)))
+        if lease.value:
+            m = n.value
+            blk = ResultLease(self.ctx, lease.value, p.value, m * (width + (24 if with_codes else 8)))
+            words = blk.array(0, m, "S%d" % width)
+            counts = blk.array(m * width, m, np.uint64)
+            if not with_codes:
+                return words, counts, None, None
+            return words, counts, blk.array(m * (width + 8), m, np.uint64), blk.array(m * (width + 16), m, np.uint64)
         self.ctx.check(self.ctx.lib.dampr_table_fetch_words(self.ctx.h, self.h, None, int(mode), int(width), None,
                                                             None, None, None, 0, C.byref(n)))
         m = n.value
@@ -821,6 +887,7 @@ def host_join_tsv(columns, prefix=None, first=0, max_files=16, col_pre=None, row
     out_len = C.c_uint64(0)
     if prefix is not None:
         nf = C.c_uint32(0)
+        _apply_result_cache()
         if col_pre is not None:
             # formatted rows (sink_json): a byte string in front of every column, row_end instead of the newline
             pre = (C.c_char_p * k)(*[bytes(x) for x in col_pre])
@@ -840,6 +907,21 @@ def host_join_tsv(columns, prefix=None, first=0, max_files=16, col_pre=None, row
     if rc:
         raise DeviceError("dampr_host_join_tsv failed (%d)" % rc)
     return out
+
+
+def host_sink_timings():
+    """Host-clock split of the last native sink call, milliseconds: the calling thread's dictionary preparation, then
+    the largest value over the writer threads of the start delay, open(), row formatting, write() and close()."""
+    out = (C.c_double * 6)()
+    load_library().dampr_host_sink_timings(out)
+    return dict(zip(("prep", "start", "open", "format", "write", "close"), out))
+
+
+def host_pool_threads():
+    """threads the library's host worker pool has started so far in this process"""
+    n = C.c_uint64(0)
+    load_library().dampr_host_pool_threads(C.byref(n))
+    return n.value
 
 
 def host_unique_small(col, table=1 << 20, with_rows=False):

@@ -137,6 +137,9 @@ class B200Runner(object):
             if not isinstance(stage, GSink):
                 produced.append(stage.output)
         plan.forget_count_dictionary()
+        # the scans of this execution hold the runner: dropped here, their result arrays (page-locked leases of the
+        # context's result arena) are released now and not at some later garbage collection
+        self.__dict__.pop("_scan_cache", None)
         ret = []
         keep = set()
         for src in outputs:

@@ -44,6 +44,9 @@ device_arena_bytes = None
 # (its pages are then already mapped: no page faults on the way out, nothing to unmap at the end);
 # spill.release_host_arena() returns it to the OS
 host_spill_cache_bytes = 96 << 30
+# page-locked host memory a device context keeps for result downloads (the token table, the count dictionary), and
+# the bound on the sink's kept formatting buffers; a result larger than this is downloaded into pageable memory
+host_result_cache_bytes = 64 << 20
 # build of the tokenise kernel the scans start with: CTAs per SM it is sized for (4, 3 or 2; lines with more
 # distinct tokens than a build remembers are retried on the 2-CTA build, see plan.TextScan.run)
 text_kernel_ctas = 4

@@ -65,6 +65,13 @@ const char *dampr_last_error(dampr_ctx *ctx);
 int32_t dampr_ctx_timings(dampr_ctx *ctx, double *out_ms, int32_t *out_ids, int32_t cap, int32_t *n);
 int32_t dampr_ctx_timings_reset(dampr_ctx *ctx);
 int32_t dampr_ctx_timing_enable(dampr_ctx *ctx, int32_t on);
+/* Page-locked result memory. Every context keeps an arena of cudaHostAlloc blocks that results are downloaded
+ * into. A lease is a block of at least `bytes` that stays the caller's until it is released, whatever else the
+ * context is used for meanwhile; released blocks are reused and only returned to the system while the arena holds
+ * more than dampr_set_option("host_result_cache_bytes") (default 64 MB). *lease == 0 and *host_ptr == NULL: no
+ * block (bytes == 0, more than that option, or out of page-locked memory). */
+int32_t dampr_result_lease(dampr_ctx *ctx, uint64_t bytes, void **host_ptr, uint64_t *lease);
+int32_t dampr_result_release(dampr_ctx *ctx, uint64_t lease);
 /* free / total device memory: the arena the spill trigger compares against (replaces the RSS
  * polling of InterpolativeMemoryChecker, memory.py:72-113) */
 int32_t dampr_ctx_mem_info(dampr_ctx *ctx, uint64_t *free_bytes, uint64_t *total_bytes);
@@ -269,6 +276,13 @@ int32_t dampr_table_fetch(dampr_ctx *ctx, dampr_table *t, uint64_t *codes, uint6
 int32_t dampr_table_fetch_words(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, int32_t mode,
                                 uint32_t width, uint8_t *words, uint64_t *counts, uint64_t *codes,
                                 uint64_t *reps, uint64_t cap, uint64_t *n);
+/* dampr_table_fetch_words in one call, into a page-locked block leased from the context's result arena:
+ * *host_ptr = words[*n * width] | counts[*n] and, with_codes != 0, | codes[*n] | reps[*n]. The block is the caller's
+ * until dampr_result_release(ctx, *lease). *lease == 0 with *n > 0: the arena gave no block (the result is larger
+ * than the "host_result_cache_bytes" option, or page-locked memory ran out) and nothing was fetched. */
+int32_t dampr_table_fetch_words_leased(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, int32_t mode,
+                                       uint32_t width, int32_t with_codes, void **host_ptr, uint64_t *lease,
+                                       uint64_t *n);
 /* device pointer and length of the count column the last dampr_table_fetch_words downloaded, in the same row
  * order; it stays valid until the table is cleared, fetched again or destroyed (*n = 0 after a clear) */
 int32_t dampr_table_extracted_counts(dampr_ctx *ctx, dampr_table *t, uint64_t *dev_ptr, uint64_t *n);
@@ -281,6 +295,11 @@ int32_t dampr_table_extracted_counts(dampr_ctx *ctx, dampr_table *t, uint64_t *d
 int32_t dampr_count_dictionary(dampr_ctx *ctx, const uint64_t *counts, uint64_t n, uint32_t stride,
                                const int64_t *extra, uint32_t n_extra, int64_t *uniq, uint32_t *inv,
                                uint32_t *rows, uint64_t *n_uniq);
+/* the same into a leased block: *host_ptr = uniq[*n_uniq] (int64) | inv[n + n_extra] (uint32) | rows[*n_uniq]
+ * (uint32). *lease == 0 with *n_uniq > 0: the arena gave no block and nothing was downloaded. */
+int32_t dampr_count_dictionary_leased(dampr_ctx *ctx, const uint64_t *counts, uint64_t n, uint32_t stride,
+                                      const int64_t *extra, uint32_t n_extra, void **host_ptr, uint64_t *lease,
+                                      uint64_t *n_uniq);
 /* the same decoding for a kv whose keys are token codes (an exchanged / merged run): exact codes ->
  * words_host[i*width ..], hashed codes -> all-NUL (the caller patches them from their strings) */
 int32_t dampr_kv_decode_words(dampr_ctx *ctx, dampr_kv *kv, int32_t mode, uint32_t width,
@@ -305,6 +324,13 @@ int32_t dampr_host_sink_tsv(const char *prefix, uint32_t first_index, uint32_t m
                             int32_t ncols, const int32_t *kinds, const void *const *ptrs,
                             const uint32_t *widths, const void *const *aux, const void *const *aux2,
                             uint64_t *out_len, uint32_t *n_files);
+/* host-clock split of the last dampr_host_sink_tsv / dampr_host_sink_fmt call in this process, milliseconds:
+ * out_ms[0] dictionary preparation on the calling thread, then the largest value over the writer threads of
+ * [1] the delay before the thread started, [2] open(), [3] row formatting, [4] write(), [5] close() */
+int32_t dampr_host_sink_timings(double *out_ms);
+/* threads the library's host worker pool has started so far in this process (the sink, dampr_host_join_tsv and
+ * dampr_host_unique_small share one pool of at most 16, parked between calls and joined at exit) */
+int32_t dampr_host_pool_threads(uint64_t *started);
 /* the same part files with col_pre[c] (NUL-terminated, may be empty) written in front of column c and row_end in
  * place of the newline, no separators of its own: the lines of sink_json (json.dumps(value) per record,
  * dampr.py:531-539) are col_pre = `["`, `", `, `, ` ... and row_end = `]\n` */

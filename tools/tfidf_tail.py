@@ -1,4 +1,5 @@
-"""Where the serial tail of the TF-IDF step goes: python tools/tfidf_tail.py [--gb 10] [--steps 5] [--warmup 2]
+"""Where the serial tail of the TF-IDF step goes:
+python tools/tfidf_tail.py [--gb 10] [--steps 5] [--warmup 2] [--source resident|host]
 
 Runs bench.tfidf_job on text already resident in HBM (the bench's corpus: Zipf(1.1), V = 1e6, seed 1234) and reports
 the wall milliseconds of every phase after the tokenise kernel. Each phase is a call of the engine wrapped here and
@@ -10,9 +11,18 @@ closed by a device synchronise, so a phase holds its own kernels and copies and 
   download            words and counts to the host (fetch_words wall time minus the kernel)
   df_dictionary       distinct document frequencies, their inverse and one row each
   idf_eval            the rest of the cross stage: the idf of every distinct document frequency
-  sink_write          the part-file writes alone: the same bytes written once more after the step, one thread per file
-  sink_format         the native sink (format + part-file writes) minus sink_write
+  sink                the native sink: dictionary formatting, row formatting and the part-file writes
+  rewrite             not part of the step, for scale: the same bytes written once more afterwards from Python, one
+                      thread per file
+  sink.*              the library's own host clocks inside that sink call (dampr_host_sink_timings): dictionary
+                      preparation on the calling thread, then the largest value any writer thread saw for its start
+                      delay, open(), row formatting, write() and close()
   other               the step's wall time minus every phase above: Python planning, frames, stage glue
+
+--source host takes the text from page-locked host memory, as the headline does. The chunked upload and the tokenise
+launches that trail it are then one phase, `ingest`, which ends when the table's counters have arrived (the first
+point at which the host knows the last launch is done); `tokenise` and `stats` are not reported apart, and the tail
+is everything after `ingest`.
 
 The step times printed last are taken without the wrappers. Prints one JSON line on stdout."""
 import argparse
@@ -35,7 +45,7 @@ from dampr_b200 import Dampr, synth
 from dampr_b200 import device as dev
 from dampr_b200 import plan
 from dampr_b200 import runner as runner_mod
-from dampr_b200.plan import DeviceText
+from dampr_b200.plan import DeviceText, MemoryText
 
 
 def gpu_name_and_power():
@@ -75,9 +85,12 @@ class Phases(object):
                 ph.add(name, 1e3 * (time.perf_counter() - t0))
         setattr(owner, attr, timed)
 
-    def install(self):
-        self.wrap(dev.Table, "count", "tokenise")
-        self.wrap(dev.Table, "stats", "stats")
+    def install(self, host):
+        if host:
+            self.wrap(plan.TextScan, "_ingest", "ingest")
+        else:
+            self.wrap(dev.Table, "count", "tokenise")
+            self.wrap(dev.Table, "stats", "stats")
         self.wrap(dev.Table, "fetch_words", "fetch_words")
         # the df dictionary: built on the host, or handed over from the device (Ctx.count_dictionary)
         self.wrap(plan, "unique_inverse_rows", "df_dictionary")
@@ -96,18 +109,26 @@ def main():
     ap.add_argument("--vocab", type=int, default=1000000)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--source", choices=("resident", "host"), default="resident")
     args = ap.parse_args()
+    host = args.source == "host"
 
     ctx = runner_mod.get_ctx()
     vocab, cdf = synth.make_vocab(args.vocab), synth.make_cdf(args.vocab)
     tb = ctx.synth_text(1234, int(int(args.gb * 1e9) / bench.MEAN_LINE), vocab[0], vocab[1], cdf)
+    if host:
+        pin = dev.PinnedBuffer(tb.n)
+        ctx.check(ctx.lib.dampr_textbuf_download(ctx.h, tb.h, 0, pin.array.ctypes.data, tb.n))
+        source = MemoryText(pin.array[:tb.n])
+    else:
+        source = DeviceText(tb)
     out_root = tempfile.mkdtemp(prefix="dampr_tail_")
     rctx = runner_mod.get_ctx()
 
     def step(i, keep=False):
         d = os.path.join(out_root, "o%d" % i)
         t0 = time.perf_counter()
-        bench.tfidf_job(Dampr, DeviceText(tb), d)
+        bench.tfidf_job(Dampr, source, d)
         ms = 1e3 * (time.perf_counter() - t0)
         if not keep:
             shutil.rmtree(d, ignore_errors=True)
@@ -145,7 +166,7 @@ def main():
         rows = []
         for i in range(args.steps):
             ph = Phases(rctx)
-            ph.install()
+            ph.install(host)
             rctx.timings_reset()
             try:
                 total, d = step(i, keep=True)
@@ -153,13 +174,21 @@ def main():
                 ph.uninstall()
             extract = sum(ms for name, ms in rctx.timings() if name == "table_extract")
             write, out_bytes = rewrite(d)
+            sink_split = dev.host_sink_timings()
             m = ph.ms
-            r = {"tokenise": m.get("tokenise", 0.0), "stats": m.get("stats", 0.0), "extract_decode": extract,
-                 "download": m.get("fetch_words", 0.0) - extract, "df_dictionary": m.get("df_dictionary", 0.0),
-                 "idf_eval": m.get("cross", 0.0) - m.get("df_dictionary", 0.0),
-                 "sink_format": m.get("sink", 0.0) - write, "sink_write": write}
-            r["tail"] = sum(v for k, v in r.items() if k != "tokenise")
-            r["other"] = total - r["tokenise"] - r["tail"]
+            head = "ingest" if host else "tokenise"
+            r = {head: m.get(head, 0.0)}
+            if not host:
+                r["stats"] = m.get("stats", 0.0)
+            r.update({"extract_decode": extract,
+                      "download": m.get("fetch_words", 0.0) - extract, "df_dictionary": m.get("df_dictionary", 0.0),
+                      "idf_eval": m.get("cross", 0.0) - m.get("df_dictionary", 0.0),
+                      "sink": m.get("sink", 0.0)})
+            r["tail"] = sum(v for k, v in r.items() if k != head)
+            r["other"] = total - r[head] - r["tail"]
+            r["tail_with_other"] = total - r[head]
+            r["rewrite"] = write
+            r.update(("sink." + k, v) for k, v in sink_split.items())
             r["step_profiled"] = total
             rows.append(r)
         plain = [step(100 + i)[0] for i in range(args.steps)]
@@ -170,8 +199,10 @@ def main():
     print("phase            median ms   (every step)", file=sys.stderr)
     for k in keys:
         print("  %-16s %8.2f   %s" % (k, med[k], [round(r[k], 1) for r in rows]), file=sys.stderr)
+    print("  gpu: %s" % gpu_name_and_power(), file=sys.stderr)
     print("  step (no wrappers) %s ms" % [round(x, 1) for x in plain], file=sys.stderr)
-    print(json.dumps({"gpu": gpu_name_and_power(), "gb": args.gb, "vocab": args.vocab, "steps": args.steps,
+    print(json.dumps({"gpu": gpu_name_and_power(), "source": args.source, "gb": args.gb, "vocab": args.vocab,
+                      "steps": args.steps,
                       "median_ms": med, "step_ms_unwrapped": [round(x, 2) for x in plain],
                       "sink_bytes": out_bytes}))
     return 0
