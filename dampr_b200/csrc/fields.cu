@@ -40,6 +40,13 @@
 // field, the slots unrolled at compile time so the bounds stay in registers. The predicates are then evaluated in
 // chain order: the first false one drops the line before its key or value is parsed (a hole in record mode); one
 // the device cannot decide sends the line to the host, whose Python filters decide or raise.
+//
+// WS (`line.split()`, DAMPR_FIELD_SEP_WS, a compile-time parameter, so the single-byte scans compile as before): the
+// separator mask becomes the str.split() whitespace mask (0x09-0x0D, 0x1C-0x20; '\r' only reaches it under
+// cr_is_data, otherwise the line is the host's). A field starts at a non-whitespace byte whose previous byte is
+// whitespace or lies before the line (the class of the last byte is carried across the 4-byte steps), and ends at
+// the next whitespace byte or the line end. Pass 1 counts the starts (the field count: 0 for a blank line, so every
+// index is missing), pass 2 walks the class changes: change 2i opens field i, change 2i + 1 closes it.
 #include "common.cuh"
 #include "fparse.cuh"
 
@@ -121,12 +128,19 @@ __device__ __forceinline__ u32 eq7(u32 x7, u32 k) {  // bit 7 of each byte set i
     return ~(z + 0x7F7F7F7Fu) & 0x80808080u;
 }
 
-// masks (bit 7 of each byte) of the 4 bytes of w: newline, separator, byte the device does not take
+__device__ __forceinline__ u32 ge7(u32 x7, u32 k) {  // bit 7 of each byte set iff the (7-bit) byte >= k
+    return (x7 + (0x80u - k) * 0x01010101u) & 0x80808080u;
+}
+
+// masks (bit 7 of each byte) of the 4 bytes of w: newline, separator (WS: str.split() whitespace), byte the device
+// does not take
+template <bool WS>
 __device__ __forceinline__ void classify(u32 w, u32 sep, bool cr_data, u32 &nl, u32 &sp, u32 &bad) {
     const u32 hi = w & 0x80808080u;
     const u32 x7 = w & 0x7F7F7F7Fu;
     nl = eq7(x7, 0x0Au) & ~hi;
-    sp = eq7(x7, sep) & ~hi;
+    if constexpr (WS) sp = ((ge7(x7, 0x09u) & ~ge7(x7, 0x0Eu)) | (ge7(x7, 0x1Cu) & ~ge7(x7, 0x21u))) & ~hi;
+    else sp = eq7(x7, sep) & ~hi;
     bad = hi | (eq7(x7, 0u) & ~hi);
     if (!cr_data) bad |= eq7(x7, 0x0Du) & ~hi;
 }
@@ -302,8 +316,9 @@ __global__ void __launch_bounds__(SCAN_THREADS) fields_tile_scan_kernel(u64 *til
     if (tid == 0) *run = carry;
 }
 
-// the kernel body over the tiles of [own_lo, own_hi); where: the predicates of a WHERE scan
-template <int VK, int MODE, bool WHERE>
+// the kernel body over the tiles of [own_lo, own_hi); where: the predicates of a WHERE scan; WS: split on runs of
+// whitespace (`line.split()`) instead of the separator byte
+template <int VK, int MODE, bool WHERE, bool WS>
 __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi,
                                              const FieldsView &tab, const RecView &rv, const WhereView *where) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -394,21 +409,28 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
         for (u32 li = tid; li < nst; li += F_THREADS) {
             const u32 q = s.starts[li];                       // window position of the first byte
             const u32 lim = min(q + (u32)F_HALO, (u32)F_WIN);  // the line's newline must lie before lim
-            // pass 1: terminator, separators, bytes the device does not take
+            // pass 1: terminator, separators (WS: field starts), bytes the device does not take
             u32 p4 = q & ~3u;
             u32 nsep = 0, end = 0xFFFFFFFFu;
             bool bad = false;
             u32 skip = q & 3u;
+            u32 prev = 0x80000000u;   // WS: whitespace mask of the previous 4 bytes (the byte before q is whitespace)
             for (; p4 < lim; p4 += 4) {
                 const u32 w = *reinterpret_cast<const u32 *>(s.text + p4);
                 u32 nl, sp, bd;
-                classify(w, tab.sep, cr_data, nl, sp, bd);
+                classify<WS>(w, tab.sep, cr_data, nl, sp, bd);
                 if (skip) {
                     const u32 keep = ~((1u << (8 * skip)) - 1u);
                     nl &= keep;
-                    sp &= keep;
+                    if constexpr (WS) sp |= ~keep & 0x80808080u;   // the bytes before q count as whitespace
+                    else sp &= keep;
                     bd &= keep;
                     skip = 0;
+                }
+                if constexpr (WS) {   // field starts: non-whitespace after whitespace
+                    const u32 ws = sp;
+                    sp = ~ws & ((ws << 8) | (prev >> 24)) & 0x80808080u;
+                    prev = ws;
                 }
                 if (nl) {
                     const u32 b = ((u32)__ffs(nl) - 1u) >> 3;
@@ -429,7 +451,7 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
             u64 code = 0, rep = ~0ULL;
             if (!to_host) {
                 // resolve the field indices (Python semantics: negative counts from the end)
-                const int nf = (int)nsep + 1;
+                const int nf = WS ? (int)nsep : (int)nsep + 1;
                 const int ki = tab.key_field < 0 ? tab.key_field + nf : tab.key_field;
                 const bool one = tab.val_field == DAMPR_FIELD_VAL_ONE;
                 const int vi = one ? 0 : (tab.val_field < 0 ? tab.val_field + nf : tab.val_field);
@@ -437,9 +459,10 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                 if (!WHERE && kv_missing) {
                     to_host = true;   // IndexError: Python raises it
                 } else {
-                    // pass 2: field bounds (a separator at window position p closes field f and opens f + 1)
-                    u32 ks = (ki == 0) ? q : 0xFFFFFFFFu, ke = (ki == nf - 1) ? end : 0xFFFFFFFFu;
-                    u32 vs = (vi == 0) ? q : 0xFFFFFFFFu, ve = (vi == nf - 1) ? end : 0xFFFFFFFFu;
+                    // pass 2: field bounds (a separator at window position p closes field f and opens f + 1; WS:
+                    // every field opens at a class change, the last one may run to the line end)
+                    u32 ks = (!WS && ki == 0) ? q : 0xFFFFFFFFu, ke = (ki == nf - 1) ? end : 0xFFFFFFFFu;
+                    u32 vs = (!WS && vi == 0) ? q : 0xFFFFFFFFu, ve = (vi == nf - 1) ? end : 0xFFFFFFFFu;
                     int need = max(ki, vi) + 1;   // separators to visit
                     // WHERE: predicate j's field is pi[j] (-1: none, IndexError in Python), its bounds [ps[j], pe[j])
                     int pi[WHERE ? P_MAX : 1];
@@ -454,39 +477,80 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                                 if (i >= nf) i = -1;
                             }
                             pi[j] = i < 0 ? -1 : i;
-                            ps[j] = pi[j] == 0 ? q : 0xFFFFFFFFu;
+                            ps[j] = !WS && pi[j] == 0 ? q : 0xFFFFFFFFu;
                             pe[j] = pi[j] == nf - 1 ? end : 0xFFFFFFFFu;
                             need = max(need, pi[j] + 1);
                         }
                     }
                     int f = 0;
                     skip = q & 3u;
-                    for (p4 = q & ~3u; f < need && p4 < end; p4 += 4) {
-                        const u32 w = *reinterpret_cast<const u32 *>(s.text + p4);
-                        u32 nl, sp, bd;
-                        classify(w, tab.sep, cr_data, nl, sp, bd);
-                        if (skip) {
-                            sp &= ~((1u << (8 * skip)) - 1u);
-                            skip = 0;
-                        }
-                        while (sp && f < need) {
-                            const u32 p = p4 + (((u32)__ffs(sp) - 1u) >> 3);
-                            sp &= sp - 1;
-                            if (p >= end) break;
-                            if (f == ki) ke = p;
-                            if (f == vi) ve = p;
-                            if constexpr (WHERE) {
-#pragma unroll
-                                for (int j = 0; j < P_MAX; ++j)
-                                    if (f == pi[j]) pe[j] = p;
+                    if constexpr (WS) {
+                        // f counts class changes: change 2i opens field i (its first byte), 2i + 1 closes it (the
+                        // whitespace byte after it)
+                        prev = 0x80000000u;
+                        for (p4 = q & ~3u; f < 2 * need && p4 < end; p4 += 4) {
+                            const u32 w = *reinterpret_cast<const u32 *>(s.text + p4);
+                            u32 nl, ws, bd;
+                            classify<true>(w, tab.sep, cr_data, nl, ws, bd);
+                            if (skip) {
+                                ws |= ((1u << (8 * skip)) - 1u) & 0x80808080u;
+                                skip = 0;
                             }
-                            ++f;
-                            if (f == ki) ks = p + 1;
-                            if (f == vi) vs = p + 1;
-                            if constexpr (WHERE) {
+                            u32 ch = (ws ^ ((ws << 8) | (prev >> 24))) & 0x80808080u;
+                            prev = ws;
+                            while (ch && f < 2 * need) {
+                                const u32 p = p4 + (((u32)__ffs(ch) - 1u) >> 3);
+                                ch &= ch - 1;
+                                if (p >= end) break;
+                                const int fi = f >> 1;
+                                if (f & 1) {
+                                    if (fi == ki) ke = p;
+                                    if (fi == vi) ve = p;
+                                    if constexpr (WHERE) {
 #pragma unroll
-                                for (int j = 0; j < P_MAX; ++j)
-                                    if (f == pi[j]) ps[j] = p + 1;
+                                        for (int j = 0; j < P_MAX; ++j)
+                                            if (fi == pi[j]) pe[j] = p;
+                                    }
+                                } else {
+                                    if (fi == ki) ks = p;
+                                    if (fi == vi) vs = p;
+                                    if constexpr (WHERE) {
+#pragma unroll
+                                        for (int j = 0; j < P_MAX; ++j)
+                                            if (fi == pi[j]) ps[j] = p;
+                                    }
+                                }
+                                ++f;
+                            }
+                        }
+                    } else {
+                        for (p4 = q & ~3u; f < need && p4 < end; p4 += 4) {
+                            const u32 w = *reinterpret_cast<const u32 *>(s.text + p4);
+                            u32 nl, sp, bd;
+                            classify<false>(w, tab.sep, cr_data, nl, sp, bd);
+                            if (skip) {
+                                sp &= ~((1u << (8 * skip)) - 1u);
+                                skip = 0;
+                            }
+                            while (sp && f < need) {
+                                const u32 p = p4 + (((u32)__ffs(sp) - 1u) >> 3);
+                                sp &= sp - 1;
+                                if (p >= end) break;
+                                if (f == ki) ke = p;
+                                if (f == vi) ve = p;
+                                if constexpr (WHERE) {
+#pragma unroll
+                                    for (int j = 0; j < P_MAX; ++j)
+                                        if (f == pi[j]) pe[j] = p;
+                                }
+                                ++f;
+                                if (f == ki) ks = p + 1;
+                                if (f == vi) vs = p + 1;
+                                if constexpr (WHERE) {
+#pragma unroll
+                                    for (int j = 0; j < P_MAX; ++j)
+                                        if (f == pi[j]) ps[j] = p + 1;
+                                }
                             }
                         }
                     }
@@ -598,24 +662,27 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
     if (tid == 0 && s.flags) atomicOr(&tab.stats[S_FLAGS], (u64)s.flags);
 }
 
-// the plain scan (WHERE false) and the WHERE scan, whose predicates are read in place from the parameters
-template <int VK, int MODE, bool WHERE>
+// the plain scan (WHERE false) and the WHERE scan, whose predicates are read in place from the parameters; WS: the
+// `line.split()` build
+template <int VK, int MODE, bool WHERE, bool WS>
 __global__ void __launch_bounds__(F_THREADS)
 text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv) {
     static_assert(!WHERE, "a WHERE scan takes its predicates");
-    fields_tiles<VK, MODE, false>(text, n, own_lo, own_hi, tab, rv, nullptr);
+    static_assert(!WS || MODE != M_COUNT, "the count pass only looks at line starts");
+    fields_tiles<VK, MODE, false, WS>(text, n, own_lo, own_hi, tab, rv, nullptr);
 }
 
-template <int VK, int MODE, bool WHERE>
+template <int VK, int MODE, bool WHERE, bool WS>
 __global__ void __launch_bounds__(F_THREADS)
 text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv,
                    const __grid_constant__ WhereView where) {
     static_assert(WHERE, "a plain scan takes no predicates");
-    fields_tiles<VK, MODE, true>(text, n, own_lo, own_hi, tab, rv, &where);
+    fields_tiles<VK, MODE, true, WS>(text, n, own_lo, own_hi, tab, rv, &where);
 }
 
-// one kernel over the tiles of [own_lo, own_hi); WHERE: the build that applies the predicates *wh
-template <int VK, int MODE, bool WHERE = false>
+// one kernel over the tiles of [own_lo, own_hi); WHERE: the build that applies the predicates *wh; WS: the
+// whitespace-split build
+template <int VK, int MODE, bool WHERE = false, bool WS = false>
 int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const FieldsView &tv, const RecView &rv,
                   int timer, const WhereView *wh = nullptr) {
     const size_t smem = sizeof(SmemF);
@@ -623,12 +690,13 @@ int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, con
     u64 grid = (u64)ctx->num_sms * 4;
     if (grid > ntiles) grid = ntiles;
     if constexpr (WHERE) {
-        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, WhereView) = text_fields_kernel<VK, MODE, true>;
+        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, WhereView) =
+            text_fields_kernel<VK, MODE, true, WS>;
         CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         ScopedTimer tm(ctx, timer);
         kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *wh);
     } else {
-        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView) = text_fields_kernel<VK, MODE, false>;
+        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView) = text_fields_kernel<VK, MODE, false, WS>;
         CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         ScopedTimer tm(ctx, timer);
         kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv);
@@ -681,8 +749,9 @@ int check_fields_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own
     ARG_CHECK(ctx, ctx && t && tb && spec, "null");
     ARG_CHECK(ctx, own_lo <= own_hi && own_hi <= tb->n, "ownership range outside the text");
     ARG_CHECK(ctx, (own_lo % 16) == 0, "own_lo must be a multiple of 16");
-    ARG_CHECK(ctx, spec->sep > 0 && spec->sep < 0x80 && spec->sep != '\n' && spec->sep != '\r',
-              "separator must be an ASCII byte other than NUL, '\\n' and '\\r'");
+    ARG_CHECK(ctx, spec->sep == DAMPR_FIELD_SEP_WS ||
+                       (spec->sep > 0 && spec->sep < 0x80 && spec->sep != '\n' && spec->sep != '\r'),
+              "separator must be DAMPR_FIELD_SEP_WS or an ASCII byte other than NUL, '\\n' and '\\r'");
     ARG_CHECK(ctx, spec->key_kind == DAMPR_FIELD_KEY_STR || spec->key_kind == DAMPR_FIELD_KEY_INT, "key kind");
     WhereView w;
     return where_view(ctx, spec, w);
@@ -694,14 +763,24 @@ FieldsView fields_view(dampr_table *t, const dampr_fields_spec *spec, int op) {
                       op, spec->cr_is_data ? 1u : 0u};
 }
 
-// the fold pass of one range: the plain kernel, or its WHERE build when spec holds predicates
+// the fold pass of one range under one separator class: the plain kernel, or its WHERE build when spec holds
+// predicates
+template <int VK, int MODE, bool WS>
+int launch_fold_sep(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
+                    const FieldsView &tv, const RecView &rv) {
+    if (spec->npreds == 0)
+        return launch_fields<VK, MODE, false, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS);
+    WhereView w;
+    if (int r = where_view(ctx, spec, w)) return r;
+    return launch_fields<VK, MODE, true, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w);
+}
+
+// the fold pass of one range: the separator-byte build, or the whitespace-split one under DAMPR_FIELD_SEP_WS
 template <int VK, int MODE>
 int launch_fold(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
                 const FieldsView &tv, const RecView &rv) {
-    if (spec->npreds == 0) return launch_fields<VK, MODE>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS);
-    WhereView w;
-    if (int r = where_view(ctx, spec, w)) return r;
-    return launch_fields<VK, MODE, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w);
+    if (spec->sep == DAMPR_FIELD_SEP_WS) return launch_fold_sep<VK, MODE, true>(ctx, tb, own_lo, own_hi, spec, tv, rv);
+    return launch_fold_sep<VK, MODE, false>(ctx, tb, own_lo, own_hi, spec, tv, rv);
 }
 
 }  // namespace

@@ -31,6 +31,7 @@ TOK_FLAG_CR_DATA = 0x100
 # delimited-field scans (dampr_text_fields)
 FIELD_KEY_STR, FIELD_KEY_INT = 0, 1
 FIELD_VAL_ONE = 0x7FFFFFFF
+FIELD_SEP_WS = 256   # sep: split like str.split() (runs of ASCII whitespace, no '' fields)
 FIELDS_HALO = 65536
 # WHERE predicates of a field scan (dampr_field_pred): kinds, comparisons, limits per call
 PRED_STR, PRED_INT, PRED_F64, PRED_NFIELDS = range(4)
@@ -72,9 +73,9 @@ class FieldsSpec(C.Structure):
 
 
 def fields_spec(spec, cr_is_data, preds):
-    """dampr_fields_spec of spec = (sep byte, key field, key kind, value field or FIELD_VAL_ONE, op) and the WHERE
-    predicates preds = [(PRED_*, field, CMP_*, constants)]: constants a tuple of str (PRED_STR), int (PRED_INT,
-    PRED_NFIELDS) or one float (PRED_F64). The returned structure keeps its constant arrays alive."""
+    """dampr_fields_spec of spec = (sep byte or FIELD_SEP_WS, key field, key kind, value field or FIELD_VAL_ONE, op)
+    and the WHERE predicates preds = [(PRED_*, field, CMP_*, constants)]: constants a tuple of str (PRED_STR), int
+    (PRED_INT, PRED_NFIELDS) or one float (PRED_F64). The returned structure keeps its constant arrays alive."""
     sep, kf, kind, vf, op = spec
     arr = (FieldPred * max(1, len(preds)))()
     keep = [arr]
@@ -580,8 +581,8 @@ class Table(object):
         self.ctx.check(self.ctx.lib.dampr_text_count(self.ctx.h, self.h, tb.h, int(lo), int(hi), m))
 
     def fields(self, tb, lo, hi, spec, cr_is_data=False, preds=()):
-        """Fold the delimited fields of the lines starting in [lo, hi): spec = (sep byte, key field, key kind,
-        value field or FIELD_VAL_ONE, op); bytes up to hi + FIELDS_HALO must be uploaded. preds: the WHERE
+        """Fold the delimited fields of the lines starting in [lo, hi): spec = (sep byte or FIELD_SEP_WS, key field,
+        key kind, value field or FIELD_VAL_ONE, op); bytes up to hi + FIELDS_HALO must be uploaded. preds: the WHERE
         predicates (see fields_spec), applied in order before the key and value are read."""
         s = fields_spec(spec, cr_is_data, preds)
         self.ctx.check(self.ctx.lib.dampr_text_fields(self.ctx.h, self.h, tb.h, int(lo), int(hi), C.byref(s)))

@@ -231,12 +231,20 @@ def tokenizer_mode(fn):
 FIELD_STR, FIELD_INT, FIELD_FLOAT = "str", "int", "float"
 
 
-def _split_sep(e):
+SEP_WS = "<whitespace>"   # the separator of `x.split()`: runs of whitespace (never a one-character separator)
+
+
+def _split_sep(e, whitespace=False):
     """S if e is `x.split(S)` over the argument with a one-character ASCII separator other than '\\n', '\\r' and NUL
-    (the bytes that end or cannot appear in a device line), else None"""
-    if isinstance(e, E) and e.op == "call" and len(e.b) == 1 and isinstance(e.a, E) and e.a.op == "attr" \
+    (the bytes that end or cannot appear in a device line); with `whitespace`, SEP_WS if e is `x.split()` or
+    `x.split(None)`; else None. Keyword forms (sep=, maxsplit=) do not reach here: analyze() refuses them."""
+    if isinstance(e, E) and e.op == "call" and len(e.b) <= 1 and isinstance(e.a, E) and e.a.op == "attr" \
             and e.a.b == "split" and _is_arg(e.a.a):
+        if not e.b:
+            return SEP_WS if whitespace else None
         ok, s = _const(e.b[0])
+        if ok and s is None:
+            return SEP_WS if whitespace else None
         if ok and type(s) is str and len(s) == 1 and s.isascii() and s not in "\n\r\0":
             return s
     return None
@@ -282,14 +290,15 @@ def _is_one(e):
     return ok and type(v) is int and v == 1
 
 
-def text_fields_spec(key_fn, value_fn, split_fn=None):
+def text_fields_spec(key_fn, value_fn, split_fn=None, whitespace=False):
     """Device field-scan spec of a keyed(key_fn, value_fn) over text lines, optionally behind map(split_fn):
     (sep, key_index, key_kind, value_index, value_kind, mean) where the key is l.split(sep)[key_index] (FIELD_STR) or
     its int() (FIELD_INT), and the value is
       the constant 1                                   value_index None, FIELD_INT, mean False
       int() or float() of l.split(sep)[value_index]    FIELD_INT or FIELD_FLOAT, mean False
       mean()'s `(value(v), 1)`, value one of those     FIELD_INT or FIELD_FLOAT, mean True
-    Indices may be negative (Python's from-the-end). None for any other shape."""
+    Indices may be negative (Python's from-the-end). With `whitespace` the split may also be l.split() / l.split(None),
+    sep SEP_WS (a caller that only handles separator characters leaves it off). None for any other shape."""
     fns = [f for f in (key_fn, value_fn, split_fn) if f is not None]
     if not all(isinstance(f, types.FunctionType) and f.__code__.co_argcount == 1 for f in fns):
         return None
@@ -297,9 +306,10 @@ def text_fields_spec(key_fn, value_fn, split_fn=None):
     if ke is None or ve is None:
         return None
     if split_fn is None:
-        record = _split_sep                      # the split is inside the key / value functions
+        def record(x):                           # the split is inside the key / value functions
+            return _split_sep(x, whitespace)
     else:
-        sep = _split_sep(analyze(split_fn))
+        sep = _split_sep(analyze(split_fn), whitespace)
         if sep is None:
             return None
 
@@ -334,9 +344,10 @@ def _pred_const(e):
     return False, None
 
 
-def field_predicate(fn, record=None):
+def field_predicate(fn, record=None, whitespace=False):
     """Device WHERE predicate of a `filter(fn)` in front of a field fold, or None. `record` is None when fn takes the
     text line and splits it itself (l.split(S)), else the separator S of the map(lambda l: l.split(S)) fn runs after.
+    With `whitespace` fn's own split may also be l.split() / l.split(None) (sep SEP_WS).
     Returns (sep, kind, index, op, constants), with R the split record, for
       F op C, C op F   F = R[i] (FIELD_STR), int(R[i]) (FIELD_INT) or float(R[i]) (FIELD_FLOAT), op one of
                        == != < <= > >= (C op F comes back as F op' C); C a str for a str field, an int in int64 (not a
@@ -353,7 +364,8 @@ def field_predicate(fn, record=None):
     if e is None or e.op != "cmp":
         return None
     if record is None:
-        rec = _split_sep
+        def rec(x):
+            return _split_sep(x, whitespace)
     else:
         def rec(x):
             return record if _is_arg(x) else None

@@ -750,7 +750,7 @@ class FieldScan(TextScan):
 
     def __init__(self, runner, sources, spec, op, stage, mean, preds=()):
         TextScan.__init__(self, runner, sources, None)
-        self.spec = spec     # (separator byte, key index, key kind, value index or FIELD_VAL_ONE)
+        self.spec = spec     # (separator byte or FIELD_SEP_WS, key index, key kind, value index or FIELD_VAL_ONE)
         self.preds = preds   # the stage's filters as device WHERE predicates (device.fields_spec)
         self._where = {"preds": preds} if preds else {}
         self.filtered = 0    # lines the predicates dropped on the device
@@ -1019,10 +1019,10 @@ def _match_text_count(stage, inputs):
 
 
 def _match_text_fields(stage, inputs):
-    """filter* [map(l.split(S)) filter*] keyed(field key, 1 | int(field) | float(field)) + PartialReduceCombiner(+ |
-    min | max), or mean()'s keyed(field key, (int(field) | float(field), 1)) + component-wise (+, +), over text, each
-    filter one lowering.field_predicate on the key's separator: (sources, (sep byte, key index, key kind, value index
-    or FIELD_VAL_ONE), op, mean, device predicates) or None"""
+    """filter* [map(l.split(S) | l.split()) filter*] keyed(field key, 1 | int(field) | float(field)) +
+    PartialReduceCombiner(+ | min | max), or mean()'s keyed(field key, (int(field) | float(field), 1)) + component-wise
+    (+, +), over text, each filter one lowering.field_predicate on the key's separator: (sources, (sep byte or
+    FIELD_SEP_WS, key index, key kind, value index or FIELD_VAL_ONE), op, mean, device predicates) or None"""
     if not isinstance(stage, GMap) or len(inputs) != 1:
         return None
     src = _text_files(inputs[0])
@@ -1037,14 +1037,14 @@ def _match_text_fields(stage, inputs):
         return None
     keyed = ks[-1][1]
     at = kinds.index("map") if "map" in kinds else None
-    spec = lowering.text_fields_spec(keyed.fn, keyed.fn2, ks[at][1].fn if at is not None else None)
+    spec = lowering.text_fields_spec(keyed.fn, keyed.fn2, ks[at][1].fn if at is not None else None, whitespace=True)
     if spec is None:
         return None
     sep, ki, kkind, vi, vkind, mean = spec
     preds = []
     for i, (k, o) in enumerate(ks[:-1]):
         if k == "filter":
-            p = lowering.field_predicate(o.fn, sep if at is not None and i > at else None)
+            p = lowering.field_predicate(o.fn, sep if at is not None and i > at else None, whitespace=True)
             if p is None or p[0] != sep:
                 return None
             preds.append(_device_pred(p))
@@ -1061,7 +1061,8 @@ def _match_text_fields(stage, inputs):
         if kind not in (lowering.ADD, lowering.MIN, lowering.MAX):
             return None
         op = (_FOLD_OPS_F64 if vkind == lowering.FIELD_FLOAT else _FOLD_OPS)[kind]
-    return src, (ord(sep), ki, dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR,
+    return src, (dev.FIELD_SEP_WS if sep == lowering.SEP_WS else ord(sep), ki,
+                 dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR,
                  dev.FIELD_VAL_ONE if vi is None else vi), op, mean, tuple(preds)
 
 
@@ -1163,6 +1164,8 @@ def _lower_map(runner, stage, inputs, si):
                                                                       scan.host_lines)
         if preds:
             detail += " filtered=%d" % scan.filtered
+        if spec[0] == dev.FIELD_SEP_WS:
+            detail += " sep=ws"
         runner.stats.add(stage, "device text fields scan+combine", detail)
         return Frame(scan.keys, [scan.values], scalar=True, combined=True)
     if _match_line_count(stage, inputs):

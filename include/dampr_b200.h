@@ -175,9 +175,17 @@ int32_t dampr_table_stats(dampr_ctx *ctx, dampr_table *t, uint64_t stats[8]);
 int32_t dampr_table_fallback_lines(dampr_ctx *ctx, dampr_table *t, uint64_t *lines, uint64_t cap, uint64_t *n);
 /* ---- delimited-field fold over text: replaces Map.stream of `l.split(S)[i]` keys with `1` / `int()` / `float()` of `l.split(S)[j]`
  *      values (base.py:30-33) fused with ReducedWriter.add_record under +, min or max (dataset.py:100-105) -------- */
+/* Below, line.split(sep) stands for the split that spec->sep selects: a separator byte, or str.split() under
+ * DAMPR_FIELD_SEP_WS. */
 #define DAMPR_FIELD_KEY_STR 0          /* key = line.split(sep)[key_field]                                   */
 #define DAMPR_FIELD_KEY_INT 1          /* key = int(line.split(sep)[key_field])                              */
 #define DAMPR_FIELD_VAL_ONE 0x7FFFFFFF /* val_field: the value is the constant 1                             */
+/* sep: split like str.split() with no argument (line.split()): fields are the maximal runs of bytes other than ASCII
+ * whitespace (0x09-0x0D, 0x1C-0x20; '\r' only under cr_is_data, otherwise the line is the caller's). Leading and
+ * trailing whitespace make no field, no field is '', and a blank or all-whitespace line has 0 fields (every index is
+ * missing). Field indices, negative ones and DAMPR_PRED_NFIELDS count these fields. Non-ASCII whitespace is never
+ * seen: a line with a non-ASCII byte is the caller's, as under a separator byte. */
+#define DAMPR_FIELD_SEP_WS 256
 /* bytes past own_hi that must be uploaded before a dampr_text_fields call (a line longer than the kernel's window
  * is measured in global memory, up to 64 KB) */
 #define DAMPR_FIELDS_HALO 65536
@@ -209,7 +217,7 @@ typedef struct dampr_field_pred {
     const uint32_t *lens;   /* STR: their lengths in bytes                                                        */
 } dampr_field_pred;
 typedef struct dampr_fields_spec {
-    int32_t sep;        /* separator byte: ASCII, not NUL, '\n' or '\r'                                     */
+    int32_t sep;        /* separator byte: ASCII, not NUL, '\n' or '\r'; or DAMPR_FIELD_SEP_WS (line.split())  */
     int32_t key_field;  /* i of line.split(sep)[i]; negative counts from the end, as in Python              */
     int32_t key_kind;   /* DAMPR_FIELD_KEY_STR | DAMPR_FIELD_KEY_INT                                         */
     int32_t val_field;  /* j of int() / float() of line.split(sep)[j], negative from the end, or

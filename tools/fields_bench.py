@@ -7,6 +7,7 @@ page-cache-warm file, the host-map MB/s on a sample, and whether the device and 
 
     python tools/fields_bench.py [--gb 2] [--keys 1000000] [--reps 3] [--sample-mb 32] [--out DIR]
                                  [--value int|float] [--op sum|min|max|mean] [--where none|str|int|float|set]
+                                 [--sep comma|ws]
 
 --value float writes the value field as float text (even lines "%.6f", odd lines repr() of the double, right-aligned
 in a 24-byte field) and folds float(r[2]); --op picks `+` (fold_by), min / max (a_group_by().reduce) or mean(). A run
@@ -21,6 +22,10 @@ MB/s, the stats line with filtered=N, and whether the host-map sample of the fil
   int    int(r[2]) >= 0           (the signed value field: about half; --value int only)
   float  float(r[2]) >= 0         (about half)
   set    r[0] not in <64 keys>    (keeps almost every line: each one is compared with all 64 members)
+
+--sep ws writes the same rows with their fields joined by runs of 1-3 spaces or tabs instead of commas, a blank in
+front of about a quarter of them and behind another quarter (the filler field gives up the bytes, so every line keeps
+its LINE bytes), and runs the same pipelines with `l.split()`. The JSON line then also holds "sep": "ws".
 """
 import argparse
 import json
@@ -86,14 +91,49 @@ def float_text(seed, n_lines, n_keys):
     return out.reshape(-1)
 
 
+def whitespace_rows(text, seed, vwidth):
+    """the rows of csv_text / float_text (value field of vwidth bytes) rewritten in place with whitespace runs for
+    separators: [blank?] key [1-3 blanks] filler [1-3 blanks] value [blank?] '\n', LINE bytes each"""
+    rows = text.reshape(-1, LINE)
+    rng = np.random.default_rng(seed)
+    step = 1 << 20
+    for a in range(0, len(rows), step):
+        t = rows[a:a + step]
+        n = len(t)
+        key, val = t[:, 0:8].copy(), t[:, LINE - 1 - vwidth:LINE - 1].copy()
+        lead = (rng.random(n) < 0.25).astype(np.int64)
+        trail = ((rng.random(n) < 0.33) & (lead == 0)).astype(np.int64)
+        r1, r2 = rng.integers(1, 4, size=n), rng.integers(1, 4, size=n)
+        blank = np.array([ord(" "), ord("\t")], dtype=np.uint8)
+        i = np.arange(n)
+        t[:, 0] = np.where(lead == 1, ord(" "), t[:, 0])
+        for j in range(8):
+            t[i, lead + j] = key[:, j]
+        for j in range(3):
+            m = j < r1
+            t[i[m], (lead + 8 + j)[m]] = blank[rng.integers(0, 2, size=int(m.sum()))]
+        vstart = LINE - 1 - trail - vwidth
+        for j in range(vwidth):
+            t[i, vstart + j] = val[:, j]
+        for j in range(1, 4):
+            m = j <= r2
+            t[i[m], (vstart - j)[m]] = blank[rng.integers(0, 2, size=int(m.sum()))]
+        t[:, LINE - 2] = np.where(trail == 1, ord(" "), t[:, LINE - 2])
+    return text
+
+
 SET_KEYS = tuple("u%07d" % (i * 7919) for i in range(64))
 WHERE = {"str": lambda r: r[0] < "u0500000", "int": lambda r: int(r[2]) >= 0, "float": lambda r: float(r[2]) >= 0,
          "set": lambda r: r[0] not in SET_KEYS}
 
 
-def job(Dampr, src, value="int", op="sum", where="none"):
+def splitter(sep):
+    return (lambda l: l.split()) if sep == "ws" else (lambda l: l.split(","))
+
+
+def job(Dampr, src, value="int", op="sum", where="none", sep="comma"):
     conv = int if value == "int" else float
-    d = Dampr.read_input(src).map(lambda l: l.split(","))
+    d = Dampr.read_input(src).map(splitter(sep))
     if where != "none":
         d = d.filter(WHERE[where])
     if op == "mean":
@@ -103,13 +143,14 @@ def job(Dampr, src, value="int", op="sum", where="none"):
     return d.fold_by(lambda r: r[0], value=lambda r: conv(r[2]), binop=lambda a, b: a + b)
 
 
-def python_fold(sample, value, op, where="none"):
+def python_fold(sample, value, op, where="none", sep="comma"):
     """the stage as plain Python over the sample's lines: {key: result}"""
     conv = int if value == "int" else float
     keep = WHERE.get(where, lambda r: True)
+    split = splitter(sep)
     out = {}
     for l in sample.decode("ascii").split("\n")[:-1]:
-        r = l.split(",")
+        r = split(l)
         if not keep(r):
             continue
         k, v = r[0], conv(r[2])
@@ -125,11 +166,12 @@ def python_fold(sample, value, op, where="none"):
     return out
 
 
-def magnitudes(sample):
+def magnitudes(sample, sep="comma"):
     """{key: (lines, sum of |float value|)} of the sample: the scale of the sum bound"""
     mag = {}
+    split = splitter(sep)
     for l in sample.decode("ascii").split("\n")[:-1]:
-        r = l.split(",")
+        r = split(l)
         n, a = mag.get(r[0], (0, 0.0))
         mag[r[0]] = (n + 1, a + abs(float(r[2])))
     return mag
@@ -168,6 +210,7 @@ def main():
     ap.add_argument("--value", choices=("int", "float"), default="int")
     ap.add_argument("--op", choices=("sum", "min", "max", "mean"), default="sum")
     ap.add_argument("--where", choices=("none", "str", "int", "float", "set"), default="none")
+    ap.add_argument("--sep", choices=("comma", "ws"), default="comma")
     a = ap.parse_args()
     if a.where == "int" and a.value != "int":
         ap.error("--where int needs --value int (int() of a float field raises)")
@@ -179,6 +222,8 @@ def main():
     name, power = card()
     n_lines = int(a.gb * 1e9) // LINE
     text = csv_text(2026, n_lines, a.keys) if a.value == "int" else float_text(2026, n_lines, a.keys)
+    if a.sep == "ws":
+        text = whitespace_rows(text, 2027, 6 if a.value == "int" else FVAL)
     nbytes = len(text)
     pin = dev.PinnedBuffer(nbytes)
     pin.array[:] = text
@@ -190,7 +235,7 @@ def main():
     def timed(src, where="none"):
         ctx.timings_reset()
         t0 = time.perf_counter()
-        n = len(list(job(Dampr, src, a.value, a.op, where).run()))
+        n = len(list(job(Dampr, src, a.value, a.op, where, a.sep).run()))
         dt = time.perf_counter() - t0
         stages = runner_mod.LAST_STATS.stages
         assert "device text fields scan+combine" in stages[0][1], stages
@@ -221,16 +266,17 @@ def main():
     t0 = time.perf_counter()
     if default:
         host = {}
+        split = splitter(a.sep)
         for l in sample.decode("ascii").split("\n")[:-1]:
-            r = l.split(",")
+            r = split(l)
             k, v = r[0], int(r[2])
             host[k] = host[k] + v if k in host else v
     else:
-        host = python_fold(sample, a.value, a.op)
+        host = python_fold(sample, a.value, a.op, sep=a.sep)
     host_s = time.perf_counter() - t0
     spin = dev.PinnedBuffer(len(sample))
     spin.array[:] = np.frombuffer(sample, dtype=np.uint8)
-    got = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op).run())
+    got = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op, sep=a.sep).run())
 
     kernel_ms = min(m[1] for m in mem)
     res = {
@@ -255,12 +301,12 @@ def main():
         res.update({"value": a.value, "op": a.op,
                     "kernels_ms": {k: round(v, 3) for k, v in sorted(best[4].items())}})
         if a.value == "float" and a.op in ("sum", "mean"):
-            res["sample_within_bound"] = within_bound(got, host, magnitudes(sample), a.op)
+            res["sample_within_bound"] = within_bound(got, host, magnitudes(sample, a.sep), a.op)
     if a.where != "none":
         t0 = time.perf_counter()
-        whost = python_fold(sample, a.value, a.op, a.where)
+        whost = python_fold(sample, a.value, a.op, a.where, a.sep)
         whost_s = time.perf_counter() - t0
-        wgot = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op, a.where).run())
+        wgot = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op, a.where, a.sep).run())
         wk = min(m[1] for m in wmem)
         res.update({
             "where": a.where,
@@ -271,9 +317,11 @@ def main():
             "where_e2e_file_warm_MBps": round(nbytes / min(f[0] for f in wfil) / 1e6, 1),
             "where_host_map_MBps": round(len(sample) / whost_s / 1e6, 1),
             "where_sample_equal": wgot == whost if not (a.value == "float" and a.op in ("sum", "mean")) else
-            within_bound(wgot, whost, magnitudes(sample), a.op),
+            within_bound(wgot, whost, magnitudes(sample, a.sep), a.op),
             "where_stats": wmem[0][3],
         })
+    if a.sep == "ws":
+        res["sep"] = "ws"
     if a.out is None:
         shutil.rmtree(tmpdir, ignore_errors=True)
     print(json.dumps(res))
