@@ -1,8 +1,11 @@
 """Differential test against the REAL reference (Refefer/Dampr), whose results are stored (ReferenceReplay): seeded
-random DSL pipelines run through Refefer/Dampr's own
-MTRunner and through this engine's runner (on the numpy stand-in for the device, tests/fake_device.py) must
-give the same multiset of results. This pins the DSL semantics of the host layer — stage fusion, keyed
-records, combiners, joins — to the reference itself rather than to a restatement."""
+random DSL pipelines run through Refefer/Dampr's own MTRunner and through this engine's runner must give the same
+multiset of results. This pins the DSL semantics — stage fusion, keyed records, combiners, joins — to the reference
+itself rather than to a restatement. Every test runs on the numpy stand-in for the device (tests/fake_device.py, the
+`engine` fixture), which keeps the host layer covered on machines without a GPU, and again on the H100 (the
+`device_engine` fixture, the *_on_the_device tests at the end of this file), where the kernels and the device-only
+branches of the lowerings (the real tokeniser, hash_join compaction, device group order) meet the reference's
+outputs."""
 import gzip
 import hashlib
 import os
@@ -18,30 +21,105 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "dif
 
 
 class ReferenceReplay(object):
-    """`subprocess` for this module's runs of the reference ([python, "-c", driver, REF, args...]): their stdout,
-    stored in GOLDEN under a digest of driver and arguments (of paths only the last component). With
-    DAMPR_REFERENCE (a reference checkout) set, the reference runs and its output is recorded."""
+    """`subprocess` for runs of the reference ([python, "-c", driver, REF, args...]): their stdout, stored in the
+    golden file under a digest of driver and arguments (of paths only the last component). With DAMPR_REFERENCE (a
+    reference checkout) set, the reference runs and its output is recorded."""
 
-    @staticmethod
-    def run(cmd, **kw):
+    def __init__(self, golden):
+        self.golden = golden
+
+    def run(self, cmd, **kw):
         inputs = [cmd[2]] + [os.path.basename(a) if a.startswith(os.sep) else a for a in cmd[4:]]
         key = hashlib.sha256("\0".join(inputs).encode()).hexdigest()[:20]
         runs = {}
-        if os.path.exists(GOLDEN):
-            with gzip.open(GOLDEN, "rb") as f:
+        if os.path.exists(self.golden):
+            with gzip.open(self.golden, "rb") as f:
                 runs = json.loads(f.read())
         if REF:
             p = _subprocess.run(cmd, **kw)
             if p.returncode == 0:
                 runs[key] = p.stdout.strip().split("\n")[-1]
-                with gzip.GzipFile(GOLDEN, "wb", mtime=0) as f:
+                with gzip.GzipFile(self.golden, "wb", mtime=0) as f:
                     f.write(json.dumps(runs, sort_keys=True).encode())
             return p
         assert key in runs, "no recorded reference output for these inputs: record with DAMPR_REFERENCE=<checkout>"
         return _subprocess.CompletedProcess(cmd, 0, runs[key], "")
 
 
-subprocess = ReferenceReplay
+subprocess = ReferenceReplay(GOLDEN)
+
+
+def _no_text_buffer(ctx, capacity):
+    from dampr_b200.plan import NotLowerable
+    raise NotLowerable("text stages run as host maps in this test")
+
+
+class Engine(object):
+    """Where the runner's device calls go for one test: the H100 ("device") or the numpy stand-in ("fake").
+    use() installs it before a pipeline runs; hows() are the paths the last run's stages took. On the device,
+    ran_on_device() checks that kernels were launched: the stand-in takes the same planner branches and prints the
+    same paths, so only the launch count tells the two apart."""
+
+    def __init__(self, kind, monkeypatch):
+        from dampr_b200 import plan
+        self.kind, self.mp = kind, monkeypatch
+        self.seen = set()
+        monkeypatch.setattr(plan, "_BUFFERS", {})
+        self.launched = self.launches()
+
+    @property
+    def device(self):
+        return self.kind == "device"
+
+    def use(self, text=None):
+        """text="host-map": text stages run as host maps; text="scan-plumbing": through plan.TextScan (the real
+        tokeniser on the device, the stand-in tokeniser of tests/fake_device.py otherwise)"""
+        import fake_device as F
+        from dampr_b200 import plan, settings
+        from dampr_b200 import runner as runner_mod
+        if self.device:
+            if text == "host-map":
+                self.mp.setattr(plan, "_cached_textbuf", _no_text_buffer)
+            return
+        if text == "scan-plumbing":
+            self.mp.setattr(runner_mod, "_CTX", {settings.device: F.FakeTextCtx()})
+            self.mp.setattr(plan, "_pinned_ring", lambda n, b: [F.FakePinned(b) for _ in range(n)])
+        else:
+            self.mp.setattr(runner_mod, "_CTX", {settings.device: F.FakeCtx()})
+        self.mp.setattr(plan, "_BUFFERS", {})
+
+    def launches(self):
+        from dampr_b200 import runner as runner_mod
+        return runner_mod.get_ctx().launches() if self.device else 0
+
+    def hows(self):
+        """the paths of the last run's stages (also collected in self.seen)"""
+        from dampr_b200 import runner as runner_mod
+        hs = [h for _s, h, _d in runner_mod.LAST_STATS.stages]
+        self.seen.update(hs)
+        return hs
+
+    def ran_on_device(self):
+        if self.device:
+            from dampr_b200 import device as dev
+            from dampr_b200 import runner as runner_mod
+            assert isinstance(runner_mod.get_ctx(), dev.Ctx)
+            assert self.launches() > self.launched, "no kernel was launched"
+
+
+@pytest.fixture
+def engine(monkeypatch):
+    """the numpy stand-in"""
+    return Engine("fake", monkeypatch)
+
+
+@pytest.fixture
+def device_engine(monkeypatch):
+    """the H100, with fresh scan buffers that are released afterwards"""
+    from dampr_b200 import plan
+    e = Engine("device", monkeypatch)
+    yield e
+    plan.release_buffers()
 
 
 def pipelines(seed, n_cases):
@@ -81,6 +159,10 @@ def pipelines(seed, n_cases):
     return out
 
 
+# the paths of Dampr.memory pipelines: host maps, then device sorts, folds and join ranges of the key codes
+SHUFFLED = {"host-map + device shuffle", "host-map + device shuffle/combine", "device join ranges + host aggregate"}
+
+
 DRIVER = r"""
 import sys, json
 sys.path.insert(0, sys.argv[1])
@@ -94,10 +176,8 @@ print(json.dumps(res))
 """
 
 
-def test_random_pipelines_agree_with_the_reference(monkeypatch):
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+def test_random_pipelines_agree_with_the_reference(engine):
+    from dampr_b200 import Dampr
     rng = random.Random(7)
     items = [rng.randint(-50, 200) for _ in range(300)]
     srcs = pipelines(2024, 60)
@@ -108,16 +188,18 @@ def test_random_pipelines_agree_with_the_reference(monkeypatch):
                        text=True, env=env, cwd="/tmp", timeout=240)
     assert p.returncode == 0, p.stderr[-2000:]
     ref = json.loads(p.stdout.strip().split("\n")[-1])
-    monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-    monkeypatch.setattr(plan, "_BUFFERS", {})
+    engine.use()
     for src, exp in zip(srcs, ref):
         got = sorted(repr(x) for x in eval(src, {"Dampr": Dampr, "items": items}).run())
+        engine.hows()
         if ".mean(" in src:
             g = [eval(x) for x in got]
             e = [eval(x) for x in exp]
             assert len(g) == len(e) and all(a[0] == b[0] and abs(a[1] - b[1]) <= 1e-9 * max(1.0, abs(b[1])) for a, b in zip(g, e)), src
         else:
             assert got == exp, src
+    assert SHUFFLED <= engine.seen, engine.seen
+    engine.ran_on_device()
 
 
 TEXT_DRIVER = r"""
@@ -132,6 +214,16 @@ for src in json.loads(sys.argv[3]):
     res.append(sorted(repr(x) for x in r))
 print(json.dumps(res))
 """
+
+
+# the paths of text stages that read the text on the device, and how many of the pipelines of
+# test_random_text_pipelines_agree_with_the_reference and of test_directory_inputs_agree_with_the_reference take one
+# when text scans are allowed: LOWERED_PER_LINE are [^\w]+ tokenisers over text with '\r' or non-ASCII lines, which
+# only the stand-in lowers
+TEXT_SCANS = ("device text tokenise+combine", "device line count", "device text fields scan+combine")
+LOWERED_TEXT = 49
+LOWERED_PER_LINE = 12
+LOWERED_DIRECTORY = 8
 
 
 def text_pipelines(seed, n_cases, longest):
@@ -158,17 +250,17 @@ def text_pipelines(seed, n_cases, longest):
 
 
 @pytest.mark.parametrize("path_kind", ["host-map", "scan-plumbing"])
-def test_random_text_pipelines_agree_with_the_reference(path_kind, monkeypatch, tmp_path):
+def test_random_text_pipelines_agree_with_the_reference(path_kind, engine, tmp_path):
     """Text inputs with assorted chunk sizes (line ownership at chunk seams, the '' token of re.split,
     str.split) through the reference and through this engine: once with every text stage as a host map, once
-    through the lowered path's plumbing (plan.TextScan) with the stand-in tokeniser of tests/fake_device.py."""
+    through the lowered path (plan.TextScan): the real tokeniser on the device, the stand-in tokeniser of
+    tests/fake_device.py otherwise."""
     import math
     import re
-    from fake_device import FakeCtx
     from oracle import gen
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+    from dampr_b200 import Dampr
     RX = re.compile(r"[^\w]+")
+    scanned = {False: 0, True: 0}
     # '\r' and '\r\n' line ends (universal newlines) and UTF-8 text: one chunk per file, because with several
     # chunks the reference's character positions drift from its byte seeks and it yields some lines twice
     cr = b"a b\r\nCcc d_1\r\n\r\nx.y 42\r\n" * 20
@@ -187,16 +279,19 @@ def test_random_text_pipelines_agree_with_the_reference(path_kind, monkeypatch, 
                            text=True, env=env, cwd="/tmp", timeout=240)
         assert p.returncode == 0, p.stderr[-2000:]
         ref = json.loads(p.stdout.strip().split("\n")[-1])
-        if path_kind == "host-map":
-            monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-        else:
-            from fake_device import FakeTextCtx, FakePinned
-            monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeTextCtx()})
-            monkeypatch.setattr(plan, "_pinned_ring", lambda n, b: [FakePinned(b) for _ in range(n)])
-        monkeypatch.setattr(plan, "_BUFFERS", {})
+        engine.use(text=path_kind)
         for src, exp in zip(srcs, ref):
             got = sorted(repr(x) for x in eval(src, {"Dampr": Dampr, "path": path, "RX": RX, "math": math}).run())
+            per_line = "RX.split" in src and (b"\r" in data or not data.isascii())
+            scanned[per_line] += any(h.startswith(TEXT_SCANS) for h in engine.hows())
             assert got == exp, (ci, src)
+    # The [^\w]+ tokenisers of the stand-in hand lines with '\r' or non-ASCII bytes back to the host one by one and
+    # keep the rest of the scan; the device's hand the whole stage back (TF_NONASCII), where it runs as a host map.
+    if path_kind == "host-map":
+        assert scanned == {False: 0, True: 0}
+    else:
+        assert scanned == {False: LOWERED_TEXT, True: 0 if engine.device else LOWERED_PER_LINE}, scanned
+    engine.ran_on_device()
 
 
 def more_pipelines(seed, n):
@@ -227,10 +322,8 @@ def more_pipelines(seed, n):
     return out
 
 
-def test_more_random_pipelines_agree_with_the_reference(monkeypatch):
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+def test_more_random_pipelines_agree_with_the_reference(engine):
+    from dampr_b200 import Dampr
     for seed, n_items in ((3, 120), (4, 7), (5, 0)):
         rng = random.Random(seed)
         items = [rng.randint(-50, 200) for _ in range(n_items)]
@@ -241,11 +334,13 @@ def test_more_random_pipelines_agree_with_the_reference(monkeypatch):
                            text=True, env=env, cwd="/tmp", timeout=240)
         assert p.returncode == 0, p.stderr[-2000:]
         ref = json.loads(p.stdout.strip().split("\n")[-1])
-        monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-        monkeypatch.setattr(plan, "_BUFFERS", {})
+        engine.use()
         for src, exp in zip(srcs, ref):
             got = sorted(repr(x) for x in eval(src, {"Dampr": Dampr, "items": items}).run())
+            engine.hows()
             assert got == exp, (n_items, src)
+    assert SHUFFLED <= engine.seen, engine.seen
+    engine.ran_on_device()
 
 
 SINK_DRIVER = r"""
@@ -266,10 +361,8 @@ print(json.dumps(res))
 """
 
 
-def test_sinks_write_the_lines_the_reference_writes(monkeypatch, tmp_path):
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+def test_sinks_write_the_lines_the_reference_writes(engine, tmp_path):
+    from dampr_b200 import Dampr
     rng = random.Random(21)
     items = [rng.randint(-50, 200) for _ in range(150)]
     templates = [
@@ -285,8 +378,7 @@ def test_sinks_write_the_lines_the_reference_writes(monkeypatch, tmp_path):
                        capture_output=True, text=True, env=env, cwd="/tmp", timeout=240)
     assert p.returncode == 0, p.stderr[-2000:]
     ref = json.loads(p.stdout.strip().split("\n")[-1])
-    monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-    monkeypatch.setattr(plan, "_BUFFERS", {})
+    engine.use()
     for i, (src, exp) in enumerate(zip(templates, ref)):
         out = str(tmp_path / ("ours%d" % i))
         eval(src, {"Dampr": Dampr, "items": items, "out": out}).run()
@@ -294,7 +386,10 @@ def test_sinks_write_the_lines_the_reference_writes(monkeypatch, tmp_path):
         for fn in sorted(os.listdir(out)):
             with open(os.path.join(out, fn)) as f:
                 lines.extend(l.rstrip("\n") for l in f)
+        engine.hows()
         assert sorted(lines) == exp, src
+    assert {"host-map + device shuffle/combine", "host sink"} <= engine.seen, engine.seen
+    engine.ran_on_device()
 
 
 def key_type_pipelines():
@@ -312,10 +407,8 @@ def key_type_pipelines():
     return srcs
 
 
-def test_key_types_agree_with_the_reference(monkeypatch):
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+def test_key_types_agree_with_the_reference(engine):
+    from dampr_b200 import Dampr
     rng = random.Random(5)
     items = [rng.randint(-50, 200) for _ in range(90)]
     srcs = key_type_pipelines()
@@ -325,11 +418,13 @@ def test_key_types_agree_with_the_reference(monkeypatch):
                        text=True, env=env, cwd="/tmp", timeout=400)
     assert p.returncode == 0, p.stderr[-2000:]
     ref = json.loads(p.stdout.strip().split("\n")[-1])
-    monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-    monkeypatch.setattr(plan, "_BUFFERS", {})
+    engine.use()
     for src, exp in zip(srcs, ref):
         got = sorted(repr(x) for x in eval(src, {"Dampr": Dampr, "items": items}).run())
+        engine.hows()
         assert got == exp, src
+    assert SHUFFLED <= engine.seen, engine.seen
+    engine.ran_on_device()
 
 
 EXPR_DRIVER = r"""
@@ -341,12 +436,10 @@ print(json.dumps([repr(eval(src)) for src in json.loads(sys.argv[3])]))
 """
 
 
-def test_inputs_outputs_and_empty_cases_agree_with_the_reference(monkeypatch, tmp_path):
+def test_inputs_outputs_and_empty_cases_agree_with_the_reference(engine, tmp_path):
     """Dampr.json inputs, multi-output Dampr.run, read(k), empty inputs through every stage kind, topk, sample(0/1),
     first(), empty sides of inner / left joins."""
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+    from dampr_b200 import Dampr
     rng = random.Random(9)
     jpath = str(tmp_path / "j.json")
     with open(jpath, "w") as f:
@@ -383,10 +476,13 @@ def test_inputs_outputs_and_empty_cases_agree_with_the_reference(monkeypatch, tm
                        capture_output=True, text=True, env=env, cwd="/tmp", timeout=400)
     assert p.returncode == 0, p.stderr[-2000:]
     ref = json.loads(p.stdout.strip().split("\n")[-1])
-    monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-    monkeypatch.setattr(plan, "_BUFFERS", {})
+    engine.use()
     for src, exp in zip(srcs, ref):
-        assert repr(eval(src, {"Dampr": Dampr, "items": items, "jpath": jpath})) == exp, src
+        got = repr(eval(src, {"Dampr": Dampr, "items": items, "jpath": jpath}))
+        engine.hows()
+        assert got == exp, src
+    assert SHUFFLED <= engine.seen, engine.seen
+    engine.ran_on_device()
 
 
 RECS_DRIVER = r"""
@@ -398,14 +494,12 @@ print(json.dumps([sorted(repr(x) for x in eval(src).run()) for src in json.loads
 """
 
 
-def test_lowered_kv_and_frame_stages_agree_with_the_reference(monkeypatch):
+def test_lowered_kv_and_frame_stages_agree_with_the_reference(engine):
     """Binary (key, value) records through the LOWERED path of this engine — device folds / sorts of the
     columns, then the column-at-a-time frame stages (vexpr) — against the reference running the same lambdas
     record by record over the same tuples."""
     import numpy as np
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+    from dampr_b200 import Dampr
     from dampr_b200.inputs import ArrayKVInput
     rng = random.Random(13)
     keys = [rng.randint(-40, 40) for _ in range(4000)]
@@ -429,10 +523,9 @@ def test_lowered_kv_and_frame_stages_agree_with_the_reference(monkeypatch):
     K, V = np.array(keys, dtype=np.int64), np.array(vals, dtype=np.int64)
     lowered = 0
     for so, exp in zip(srcs_ours, ref):
-        monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-        monkeypatch.setattr(plan, "_BUFFERS", {})
+        engine.use()
         got = sorted(repr(x) for x in eval(so, {"Dampr": Dampr, "ArrayKVInput": ArrayKVInput, "K": K, "V": V}).run())
-        hows = [h for _s, h, _d in runner_mod.LAST_STATS.stages]
+        hows = engine.hows()
         lowered += any("column-at-a-time" in h or "frame keyed fold" in h or "device sort of frame rows" in h for h in hows)
         if ".mean(" in so:
             g, e = [eval(x) for x in got], [eval(x) for x in exp]
@@ -440,16 +533,15 @@ def test_lowered_kv_and_frame_stages_agree_with_the_reference(monkeypatch):
         else:
             assert got == exp, so
     assert lowered >= 40     # the frame stages really took the lowered path
+    engine.ran_on_device()
 
 
-def test_lowered_cross_and_sink_agree_with_the_reference(monkeypatch, tmp_path):
+def test_lowered_cross_and_sink_agree_with_the_reference(engine, tmp_path):
     """The tf-idf tail — cross_right with the 1-row total (memoised per distinct value) and the native
     sink_tsv — over a lowered count frame, against the reference's files for the same records."""
     import math
     import numpy as np
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+    from dampr_b200 import Dampr
     from dampr_b200.inputs import ArrayKVInput
     rng = random.Random(17)
     keys = [int(rng.paretovariate(1.2)) % 500 for _ in range(6000)]
@@ -476,19 +568,19 @@ print(json.dumps(sorted(lines)))
                        capture_output=True, text=True, env=env, cwd="/tmp", timeout=300)
     assert p.returncode == 0, p.stderr[-2000:]
     exp = json.loads(p.stdout.strip().split("\n")[-1])
-    monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-    monkeypatch.setattr(plan, "_BUFFERS", {})
+    engine.use()
     K, V = np.array(keys, dtype=np.int64), np.array(vals, dtype=np.int64)
     out = str(tmp_path / "ours")
     src = "Dampr.read_input(ArrayKVInput(K, V))" + tail % "Dampr.read_input(ArrayKVInput(K, V))"
     eval(src, {"Dampr": Dampr, "ArrayKVInput": ArrayKVInput, "K": K, "V": V, "math": math, "out": out}).run()
-    hows = [h for _s, h, _d in runner_mod.LAST_STATS.stages]
+    hows = engine.hows()
     assert any("memoised per distinct" in h for h in hows) and any("native frame sink" in h for h in hows), hows
     lines = []
     for fn in sorted(os.listdir(out)):
         with open(os.path.join(out, fn)) as f:
             lines.extend(l.rstrip("\n") for l in f)
     assert sorted(lines) == exp
+    engine.ran_on_device()
 
 
 TWO_DRIVER = r"""
@@ -500,13 +592,11 @@ print(json.dumps([sorted(repr(x) for x in eval(src).run()) for src in json.loads
 """
 
 
-def test_lowered_joins_probes_and_sorts_agree_with_the_reference(monkeypatch):
+def test_lowered_joins_probes_and_sorts_agree_with_the_reference(engine):
     """Reduce-side joins (inner / left) over lowered inputs, the cross_set membership probe, sorts of whole
     records and of count frames, cross_right over a frame: this engine's lowered paths vs the reference."""
     import numpy as np
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+    from dampr_b200 import Dampr
     from dampr_b200.inputs import ArrayKVInput
     rng = random.Random(23)
     keys = [rng.randint(0, 60) for _ in range(3000)]
@@ -538,27 +628,25 @@ def test_lowered_joins_probes_and_sorts_agree_with_the_reference(monkeypatch):
           "K2": np.array(k2, dtype=np.int64), "V2": np.array(v2, dtype=np.int64)}
     seen = set()
     for t, exp in zip(tmpl, ref):
-        monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-        monkeypatch.setattr(plan, "_BUFFERS", {})
+        engine.use()
         got = sorted(repr(x) for x in eval(t.format(A=A_our, B=B_our), ns).run())
-        seen.update(h for _s, h, _d in runner_mod.LAST_STATS.stages)
+        seen.update(engine.hows())
         assert got == exp, t
     for needle in ("device join ranges", "device broadcast hash build+probe", "partition+sort of whole records",
                    "device sort of frame rows", "memoised per distinct"):
         assert any(needle in h for h in seen), needle
+    engine.ran_on_device()
 
 
 @pytest.mark.parametrize("path_kind", ["host-map", "scan-plumbing"])
-def test_directory_inputs_agree_with_the_reference(path_kind, monkeypatch, tmp_path):
+def test_directory_inputs_agree_with_the_reference(path_kind, engine, tmp_path):
     """Dampr.text on a directory tree: several files laid out back to back, an empty file, files without a
     final newline, a .gz member."""
     import gzip
     import math
     import re
-    import fake_device as F
     from oracle import gen
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+    from dampr_b200 import Dampr
     RX = re.compile(r"[^\w]+")
     d = tmp_path / "corpus"
     (d / "sub" / "deep").mkdir(parents=True)
@@ -576,16 +664,18 @@ def test_directory_inputs_agree_with_the_reference(path_kind, monkeypatch, tmp_p
                        env=env, cwd="/tmp", timeout=300)
     assert p.returncode == 0, p.stderr[-2000:]
     ref = json.loads(p.stdout.strip().split("\n")[-1])
-    monkeypatch.setattr(plan, "_pinned_ring", lambda n, b: [F.FakePinned(b) for _ in range(n)])
+    scanned = 0
     for src, exp in zip(srcs, ref):
-        monkeypatch.setattr(runner_mod, "_CTX", {settings.device: F.FakeCtx() if path_kind == "host-map" else F.FakeTextCtx()})
-        monkeypatch.setattr(plan, "_BUFFERS", {})
+        engine.use(text=path_kind)
         got = sorted(repr(x) for x in eval(src, {"Dampr": Dampr, "path": str(d), "RX": RX, "math": math}).run())
+        scanned += any(h.startswith(TEXT_SCANS) for h in engine.hows())
         assert got == exp, src
+    assert scanned == (LOWERED_DIRECTORY if path_kind == "scan-plumbing" else 0)
+    engine.ran_on_device()
 
 
 @pytest.mark.parametrize("path_kind", ["host-map", "scan-plumbing"])
-def test_crlf_gzip_inputs_agree_with_the_reference(path_kind, monkeypatch, tmp_path):
+def test_crlf_gzip_inputs_agree_with_the_reference(path_kind, engine, tmp_path):
     """.gz text is read in BINARY mode by the reference (dataset.py:488-493): only '\\n' ends a line, the '\\r'
     of a CRLF file stays in the line (so the tf-idf tokeniser yields a '' token per line and 'hello world\\r'
     is the line), a lone '\\r' does not end a line. Both as a gz-only directory (stays lowered: the CR flag is
@@ -593,9 +683,7 @@ def test_crlf_gzip_inputs_agree_with_the_reference(path_kind, monkeypatch, tmp_p
     import gzip
     import math
     import re
-    import fake_device as F
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+    from dampr_b200 import Dampr
     RX = re.compile(r"[^\w]+")
     crlf = b"hello world\r\nfoo bar\r\nlone\rcr inside\r\n\r\nlast line no cr\nunterminated\r"
     for layout in ("gz-only", "mixed"):
@@ -621,26 +709,26 @@ def test_crlf_gzip_inputs_agree_with_the_reference(path_kind, monkeypatch, tmp_p
         assert p.returncode == 0, p.stderr[-2000:]
         ref = json.loads(p.stdout.strip().split("\n")[-1])
         assert repr("hello world\r") in ref[4] if layout == "gz-only" else True
-        monkeypatch.setattr(plan, "_pinned_ring", lambda n, b: [F.FakePinned(b) for _ in range(n)])
         for src, exp in zip(srcs, ref):
-            monkeypatch.setattr(runner_mod, "_CTX", {settings.device: F.FakeCtx() if path_kind == "host-map" else F.FakeTextCtx()})
-            monkeypatch.setattr(plan, "_BUFFERS", {})
+            engine.use(text=path_kind)
             got = sorted(repr(x) for x in eval(src, {"Dampr": Dampr, "path": str(d), "RX": RX, "math": math}).run())
+            hows = engine.hows()
             assert got == exp, (layout, src)
             if path_kind == "scan-plumbing" and layout == "gz-only" and "count" in src:
-                assert any("device text tokenise+combine" in h for _s, h, _d in runner_mod.LAST_STATS.stages), src
+                assert any("device text tokenise+combine" in h for h in hows), src
+            if path_kind == "host-map":
+                assert not any(h.startswith(TEXT_SCANS) for h in hows), src
+    engine.ran_on_device()
 
 
-def test_lowered_join_idioms_agree_with_the_reference(monkeypatch):
+def test_lowered_join_idioms_agree_with_the_reference(engine):
     """Columnar reduce-side joins (plan._lower_join): per-side folds (inner and left), and itertools.product over a
     right side with unique keys (many=True) — vs the reference's InnerJoin / LeftJoin (base.py:264-315). Joins whose
     aggregate is not an idiom, or whose right side has duplicate keys under product, take the generic path and
     must agree as well."""
     import itertools
     import numpy as np
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+    from dampr_b200 import Dampr
     from dampr_b200.inputs import ArrayKVInput
     rng = random.Random(41)
     keys = [rng.randint(0, 400) for _ in range(5000)]
@@ -672,28 +760,26 @@ def test_lowered_join_idioms_agree_with_the_reference(monkeypatch):
           "V": np.array(vals, dtype=np.int64), "K2": np.array(k2, dtype=np.int64), "V2": np.array(v2, dtype=np.int64)}
     hows = []
     for t, exp in zip(tmpl, ref):
-        monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-        monkeypatch.setattr(plan, "_BUFFERS", {})
+        engine.use()
         got = sorted(repr(x) for x in eval(t.format(A=A_our, B=B_our), ns).run())
-        hows.append([h for _s, h, _d in runner_mod.LAST_STATS.stages])
+        hows.append(engine.hows())
         assert got == exp, t
     for i in range(5):
         assert any("device join: per-side partition+sort+fold" in h for h in hows[i]), tmpl[i]
     assert any("device join: broadcast hash build + probe" in h for h in hows[5])
     for i in (6, 7):
         assert not any("device join:" in h for h in hows[i]), tmpl[i]
+    engine.ran_on_device()
 
 
-def test_lowered_topk_unique_prefix_agree_with_the_reference(monkeypatch):
+def test_lowered_topk_unique_prefix_agree_with_the_reference(engine):
     """The lowerings added for SURVEY §8(f)2 — topk over a frame (plan._lower_topk), group_by(...).unique() over kv
     records (plan._lower_unique), prefix / suffix / map_keys through the frame map — against the reference's own
     topk (dampr.py:621-652), unique (:727-746) and prefix / suffix (:310-340) on the same records. unique()'s value
     order inside a group is the reference's merge order, which depends on its worker scheduling: one input
     partition keeps it the input order, which is what the lowering produces."""
     import numpy as np
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+    from dampr_b200 import Dampr
     from dampr_b200.inputs import ArrayKVInput
     rng = random.Random(77)
     keys = [rng.randint(0, 300) for _ in range(6000)]
@@ -728,10 +814,9 @@ def test_lowered_topk_unique_prefix_agree_with_the_reference(monkeypatch):
     ns = {"Dampr": Dampr, "ArrayKVInput": ArrayKVInput, "K": np.array(keys, dtype=np.int64), "V": np.array(vals, dtype=np.int64)}
     hows = []
     for t, exp in zip(tmpl, ref):
-        monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-        monkeypatch.setattr(plan, "_BUFFERS", {})
+        engine.use()
         got = sorted(repr(x) for x in eval(t.format(A=A_our), ns).run())
-        hows.append([h for _s, h, _d in runner_mod.LAST_STATS.stages])
+        hows.append(engine.hows())
         assert got == exp, t
     for i in (0, 1, 2):
         assert any("device top-k candidates" in h for h in hows[i]), tmpl[i]
@@ -744,16 +829,15 @@ def test_lowered_topk_unique_prefix_agree_with_the_reference(monkeypatch):
         assert any("frame map/filter evaluated column-at-a-time" in h for h in hows[i]), (tmpl[i], hows[i])
     for i in (12, 13):
         assert any("native frame sink" in h for h in hows[i]), (tmpl[i], hows[i])
+    engine.ran_on_device()
 
 
-def test_chains_over_binary_kv_inputs_agree_with_the_reference(monkeypatch):
+def test_chains_over_binary_kv_inputs_agree_with_the_reference(engine):
     """Stages over binary (key, value) inputs that are more than a bare keyed fold — a map / filter chain in front of
     it, mean(), topk, a plain map, len() — run column-at-a-time on the two input columns (plan._lower_map: the kv
     input as a frame of (key, value) rows). Same records through the reference as Dampr.memory tuples."""
     import numpy as np
-    from fake_device import FakeCtx
-    from dampr_b200 import Dampr, settings, plan
-    from dampr_b200 import runner as runner_mod
+    from dampr_b200 import Dampr
     from dampr_b200.inputs import ArrayKVInput
     rng = random.Random(99)
     keys = [rng.randint(0, 200) for _ in range(5000)]
@@ -784,10 +868,9 @@ def test_chains_over_binary_kv_inputs_agree_with_the_reference(monkeypatch):
     ns = {"Dampr": Dampr, "ArrayKVInput": ArrayKVInput, "K": np.array(keys, dtype=np.int64), "V": np.array(vals, dtype=np.int64)}
     hows = []
     for t, exp in zip(tmpl, ref):
-        monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-        monkeypatch.setattr(plan, "_BUFFERS", {})
+        engine.use()
         got = sorted(repr(x) for x in eval(t.format(A=A_our), ns).run())
-        hows.append([h for _s, h, _d in runner_mod.LAST_STATS.stages])
+        hows.append(engine.hows())
         assert got == exp, t
     assert any("record count of a columnar input" in h for h in hows[0])
     for i in range(1, 10):
@@ -809,9 +892,89 @@ def test_chains_over_binary_kv_inputs_agree_with_the_reference(monkeypatch):
     ref2 = json.loads(p.stdout.strip().split("\n")[-1])
     ns["K"], ns["V"] = np.array(big, dtype=np.uint64), np.array(vals, dtype=np.int64)
     for i, (t, exp) in enumerate(zip(tmpl2, ref2)):
-        monkeypatch.setattr(runner_mod, "_CTX", {settings.device: FakeCtx()})
-        monkeypatch.setattr(plan, "_BUFFERS", {})
+        engine.use()
         got = sorted(repr(x) for x in eval(t.format(A=A_our), ns).run())
         assert got == exp, t
-        first = [h for _s, h, _d in runner_mod.LAST_STATS.stages][0]
+        first = engine.hows()[0]
         assert first.startswith("host-map") == (i == 3), (t, first)
+    engine.ran_on_device()
+
+
+# ---- the same tests on the H100 -----------------------------------------------------------------------------------
+PATH_KINDS = pytest.mark.parametrize("path_kind", ["host-map", "scan-plumbing"])
+
+
+@pytest.mark.gpu
+def test_random_pipelines_on_the_device(device_engine):
+    test_random_pipelines_agree_with_the_reference(device_engine)
+
+
+@pytest.mark.gpu
+@PATH_KINDS
+def test_random_text_pipelines_on_the_device(path_kind, device_engine, tmp_path):
+    test_random_text_pipelines_agree_with_the_reference(path_kind, device_engine, tmp_path)
+
+
+@pytest.mark.gpu
+def test_more_random_pipelines_on_the_device(device_engine):
+    test_more_random_pipelines_agree_with_the_reference(device_engine)
+
+
+@pytest.mark.gpu
+def test_sinks_on_the_device(device_engine, tmp_path):
+    # the recording is keyed by the name of the output directory: the one pytest gives the test above
+    out = tmp_path / "test_sinks_write_the_lines_the0"
+    out.mkdir()
+    test_sinks_write_the_lines_the_reference_writes(device_engine, out)
+
+
+@pytest.mark.gpu
+def test_key_types_on_the_device(device_engine):
+    test_key_types_agree_with_the_reference(device_engine)
+
+
+@pytest.mark.gpu
+def test_inputs_outputs_and_empty_cases_on_the_device(device_engine, tmp_path):
+    test_inputs_outputs_and_empty_cases_agree_with_the_reference(device_engine, tmp_path)
+
+
+@pytest.mark.gpu
+def test_lowered_kv_and_frame_stages_on_the_device(device_engine):
+    test_lowered_kv_and_frame_stages_agree_with_the_reference(device_engine)
+
+
+@pytest.mark.gpu
+def test_lowered_cross_and_sink_on_the_device(device_engine, tmp_path):
+    test_lowered_cross_and_sink_agree_with_the_reference(device_engine, tmp_path)
+
+
+@pytest.mark.gpu
+def test_lowered_joins_probes_and_sorts_on_the_device(device_engine):
+    test_lowered_joins_probes_and_sorts_agree_with_the_reference(device_engine)
+
+
+@pytest.mark.gpu
+@PATH_KINDS
+def test_directory_inputs_on_the_device(path_kind, device_engine, tmp_path):
+    test_directory_inputs_agree_with_the_reference(path_kind, device_engine, tmp_path)
+
+
+@pytest.mark.gpu
+@PATH_KINDS
+def test_crlf_gzip_inputs_on_the_device(path_kind, device_engine, tmp_path):
+    test_crlf_gzip_inputs_agree_with_the_reference(path_kind, device_engine, tmp_path)
+
+
+@pytest.mark.gpu
+def test_lowered_join_idioms_on_the_device(device_engine):
+    test_lowered_join_idioms_agree_with_the_reference(device_engine)
+
+
+@pytest.mark.gpu
+def test_lowered_topk_unique_prefix_on_the_device(device_engine):
+    test_lowered_topk_unique_prefix_agree_with_the_reference(device_engine)
+
+
+@pytest.mark.gpu
+def test_chains_over_binary_kv_inputs_on_the_device(device_engine):
+    test_chains_over_binary_kv_inputs_agree_with_the_reference(device_engine)
