@@ -221,6 +221,211 @@ __device__ __noinline__ int eval_pred(const WhereView &w, const PredSlot &pr, bo
     return r == (pr.cmp == DAMPR_CMP_IN);
 }
 
+// ---- JSON lines ------------------------------------------------------------------------------------------------
+constexpr int J_MAX = DAMPR_JSON_MAX_MEMBERS;
+constexpr int J_NAME = DAMPR_JSON_MAX_NAME;
+constexpr int J_DEPTH = DAMPR_JSON_MAX_DEPTH;
+static_assert(J_DEPTH <= 64, "the container stack is one u64");
+static_assert(F_WIN <= 0xFFFF, "member bounds pack two 16-bit window positions");
+
+// the JSON type of a member, 4 bits per member in one u32 (NONE: not in the line)
+enum { JT_NONE = 0, JT_STR = 1, JT_ESC = 2, JT_INT = 3, JT_FLOAT = 4, JT_OTHER = 5 };
+
+// the wanted member names of a JSON scan, passed by value in the kernel parameters
+struct JsonView {
+    u8 name[J_MAX][J_NAME];
+    u8 len[J_MAX];
+    int n;
+};
+
+// first position >= i whose byte is not an ASCII digit (the line's '\n' stops it)
+__device__ __forceinline__ u32 skip_digits(const u8 *t, u32 i) {
+    for (;;) {
+        const u32 a = i & ~3u;
+        const u32 x7 = *reinterpret_cast<const u32 *>(t + a) & 0x7F7F7F7Fu;
+        const u32 nd = ~(ge7(x7, '0') & ~ge7(x7, '9' + 1)) & 0x80808080u & (~0u << (8 * (i - a)));
+        if (nd) return a + (((u32)__ffs(nd) - 1u) >> 3);
+        i = a + 4;
+    }
+}
+
+// first position >= i whose byte is '"', '\\' or below 0x20 (the line's '\n' stops it)
+__device__ __forceinline__ u32 skip_string(const u8 *t, u32 i) {
+    for (;;) {
+        const u32 a = i & ~3u;
+        const u32 x7 = *reinterpret_cast<const u32 *>(t + a) & 0x7F7F7F7Fu;
+        const u32 sp = (eq7(x7, '"') | eq7(x7, '\\') | ~ge7(x7, 0x20u)) & 0x80808080u & (~0u << (8 * (i - a)));
+        if (sp) return a + (((u32)__ffs(sp) - 1u) >> 3);
+        i = a + 4;
+    }
+}
+
+__device__ __forceinline__ bool is_digit(u8 c) { return (u32)c - '0' <= 9u; }
+__device__ __forceinline__ bool is_hex(u8 c) { return is_digit(c) || (u32)(c | 0x20) - 'a' <= 5u; }
+
+// t[p, end) against the bytes of lit (json.loads' true / false / null)
+__device__ __forceinline__ bool lit_at(const u8 *t, u32 p, u32 end, const char *lit, u32 n) {
+    if (p + n > end) return false;
+    for (u32 i = 0; i < n; ++i)
+        if (t[p + i] != (u8)lit[i]) return false;
+    return true;
+}
+
+// the JSON string whose opening quote is at p: *e = the position of its closing quote, *esc = it holds an escape;
+// false when json.loads rejects it (a bad escape, a raw byte below 0x20, no closing quote before the line end)
+__device__ __forceinline__ bool json_string(const u8 *t, u32 p, u32 end, u32 &e, bool &esc) {
+    esc = false;
+    for (e = p + 1;;) {
+        e = skip_string(t, e);
+        if (e >= end || t[e] < 0x20) return false;
+        if (t[e] == '"') return true;
+        esc = true;
+        const u8 x = t[e + 1];
+        if (x == 'u') {
+            if (e + 6 > end || !is_hex(t[e + 2]) || !is_hex(t[e + 3]) || !is_hex(t[e + 4]) || !is_hex(t[e + 5]))
+                return false;
+            e += 6;
+        } else if (x == '"' || x == '\\' || x == '/' || x == 'b' || x == 'f' || x == 'n' || x == 'r' || x == 't') {
+            e += 2;
+        } else {
+            return false;
+        }
+    }
+}
+
+// Validate the line t[q, end) (t[end] == '\n'; every byte ASCII, not NUL, '\r' only where it is data) as one JSON
+// text whose top-level value is an object, under json.loads' grammar, and record the last occurrence of each wanted
+// top-level member: mb[j] = start | end << 16 of its value (a string's bytes between the quotes), its JT_* type in
+// bits 4j of mt. false for anything json.loads rejects (the host raises), a nesting deeper than J_DEPTH, and a
+// top-level name with an escape (it might decode to a wanted name).
+template <int JM>
+__device__ __forceinline__ bool json_line(const u8 *t, u32 q, u32 end, const JsonView &jv, u32 (&mb)[JM], u32 &mt) {
+    enum { VALUE, VALUE_OR_CLOSE, NAME, NAME_OR_CLOSE, COLON, AFTER };
+    u64 objs = 0;     // bit d - 1: the container at depth d is an object
+    int depth = 0;
+    int st = VALUE;
+    int cur = -1;     // the wanted member whose value comes next (depth 1)
+    u32 p = q;
+    while (p < end) {
+        const u8 c = t[p];
+        if (c == ' ' || c == '\t' || c == '\r') {   // '\r' is only here when it is data: JSON whitespace
+            ++p;
+            continue;
+        }
+        if (st == NAME_OR_CLOSE && c == '}') {
+            objs &= ~(1ULL << --depth);
+            st = AFTER;
+            ++p;
+            continue;
+        }
+        if (st == NAME_OR_CLOSE || st == NAME) {
+            u32 e;
+            bool esc;
+            if (c != '"' || !json_string(t, p, end, e, esc)) return false;
+            if (depth == 1) {
+                if (esc) return false;
+                const u32 len = e - p - 1;
+                cur = -1;
+#pragma unroll
+                for (int j = 0; j < JM; ++j) {
+                    if (j < jv.n && cur < 0 && len == jv.len[j]) {
+                        bool same = true;
+                        for (u32 i = 0; i < len && same; ++i) same = t[p + 1 + i] == jv.name[j][i];
+                        if (same) cur = j;
+                    }
+                }
+            }
+            p = e + 1;
+            st = COLON;
+            continue;
+        }
+        if (st == COLON) {
+            if (c != ':') return false;
+            ++p;
+            st = VALUE;
+            continue;
+        }
+        if (st == AFTER) {
+            if (depth == 0) return false;   // data after the top-level object
+            const bool obj = (objs >> (depth - 1)) & 1;
+            if (c == ',') st = obj ? NAME : VALUE;
+            else if (c == (obj ? '}' : ']')) objs &= ~(1ULL << --depth);
+            else return false;
+            ++p;
+            continue;
+        }
+        // a value (VALUE, VALUE_OR_CLOSE)
+        if (st == VALUE_OR_CLOSE && c == ']') {
+            --depth;
+            st = AFTER;
+            ++p;
+            continue;
+        }
+        if (depth == 0 && c != '{') return false;   // the top-level value is an object
+        const bool member = depth == 1 && cur >= 0;
+        u32 vs = p;
+        int ty = JT_OTHER;
+        st = AFTER;
+        if (c == '{' || c == '[') {
+            if (depth == J_DEPTH) return false;
+            if (c == '{') objs |= 1ULL << depth;
+            ++depth;
+            st = c == '{' ? NAME_OR_CLOSE : VALUE_OR_CLOSE;
+            ++p;
+        } else if (c == '"') {
+            u32 e;
+            bool esc;
+            if (!json_string(t, p, end, e, esc)) return false;
+            ty = esc ? JT_ESC : JT_STR;
+            vs = p + 1;
+            p = e;   // the bounds end at the closing quote, the scan goes on after it
+        } else if (c == '-' || is_digit(c)) {
+            u32 i = p + (c == '-');
+            if (t[i] == '0') ++i;
+            else if (is_digit(t[i])) i = skip_digits(t, i + 1);
+            else return false;
+            ty = JT_INT;
+            if (t[i] == '.') {
+                if (!is_digit(t[i + 1])) return false;
+                i = skip_digits(t, i + 2);
+                ty = JT_FLOAT;
+            }
+            if ((t[i] | 0x20) == 'e') {
+                ++i;
+                if (t[i] == '+' || t[i] == '-') ++i;
+                if (!is_digit(t[i])) return false;
+                i = skip_digits(t, i + 1);
+                ty = JT_FLOAT;
+            }
+            p = i;
+        } else {
+            const u32 n = c == 'f' ? 5u : 4u;
+            if (!lit_at(t, p, end, c == 't' ? "true" : c == 'f' ? "false" : "null", n)) return false;
+            p += n;
+        }
+        if (member) {
+#pragma unroll
+            for (int j = 0; j < JM; ++j)
+                if (j == cur) {
+                    mb[j] = vs | p << 16;
+                    mt = (mt & ~(0xFu << (4 * j))) | (u32)ty << (4 * j);
+                }
+        }
+        if (ty == JT_STR || ty == JT_ESC) ++p;   // past the closing quote
+    }
+    return st == AFTER && depth == 0;
+}
+
+// member j's entry of the packed bounds (unrolled: mb stays in registers)
+template <int JM>
+__device__ __forceinline__ u32 member_bounds(const u32 (&mb)[JM], int j) {
+    u32 b = 0;
+#pragma unroll
+    for (int i = 0; i < JM; ++i)
+        if (i == j) b = mb[i];
+    return b;
+}
+
 __device__ __forceinline__ u64 hash_bytes(const u8 *p, u32 len, u64 seed) {
     u32 h1 = (u32)seed ^ 0x811C9DC5u, h2 = (u32)(seed >> 32) ^ 0x9747B28Cu;
     for (u32 i = 0; i < len; ++i) {
@@ -316,11 +521,98 @@ __global__ void __launch_bounds__(SCAN_THREADS) fields_tile_scan_kernel(u64 *til
     if (tid == 0) *run = carry;
 }
 
+// a JSON scan's work on one line after pass 1 (t[q, end) is ASCII and ends at its '\n'): validate it, evaluate the
+// predicates on its members, then read the key and the value. Sets to_host, dropped, val, code and rep as the field
+// path does (g0: the global offset of window position 0). A kept line's key and value kinds are both reported before
+// either decides that the line is the host's.
+template <int VK, bool WHERE>
+__device__ __forceinline__ void json_fold(const u8 *t, u32 q, u32 end, u64 g0, const FieldsView &tab,
+                                          const JsonView &jv, const WhereView *where, bool &to_host, bool &dropped,
+                                          long long &val, u64 &code, u64 &rep, u64 &acc_long, u32 &flags) {
+    constexpr int JM = WHERE ? J_MAX : 2;   // the plain scan reads the key and the value only
+    u32 mb[JM];
+#pragma unroll
+    for (int j = 0; j < JM; ++j) mb[j] = 0;
+    u32 mt = 0;
+    if (!json_line<JM>(t, q, end, jv, mb, mt)) {
+        to_host = true;
+        return;
+    }
+    if constexpr (WHERE) {
+        const WhereView &wh = *where;
+        int verdict = 1;
+#pragma unroll
+        for (int j = 0; j < P_MAX; ++j) {
+            if (j < wh.n && verdict == 1) {
+                const PredSlot &pr = wh.p[j];
+                const u32 ty = (mt >> (4 * pr.field)) & 0xFu;
+                if (pr.kind == DAMPR_PRED_MEMBER) {
+                    verdict = (ty != JT_NONE) == (pr.cmp == DAMPR_CMP_IN);
+                } else {
+                    // a member of another type than the constant's, or a missing one: the host's filter decides
+                    const bool has = pr.kind == DAMPR_PRED_STR ? ty == JT_STR
+                                     : pr.kind == DAMPR_PRED_INT ? ty == JT_INT
+                                                                 : (ty == JT_INT || ty == JT_FLOAT);
+                    const u32 b = member_bounds<JM>(mb, pr.field);
+                    verdict = eval_pred(wh, pr, has, t + (b & 0xFFFFu), (b >> 16) - (b & 0xFFFFu), 0);
+                }
+            }
+        }
+        dropped = verdict == 0;
+        to_host = verdict < 0;
+        if (verdict != 1) return;
+    }
+    const u32 kt = (mt >> (4 * tab.key_field)) & 0xFu;
+    const u32 kb = member_bounds<JM>(mb, tab.key_field);
+    const u32 ks = kb & 0xFFFFu, klen = (kb >> 16) - ks;
+    bool ok;   // a missing member is a KeyError in Python: the host raises it
+    if (tab.key_int) {
+        long long kv;
+        ok = kt == JT_INT && parse_int(t + ks, klen, kv);
+        if (ok) code = (u64)kv ^ 0x8000000000000000ULL;
+        if (kt != JT_INT && kt != JT_NONE) flags |= DAMPR_TF_JSON_KEY_KIND;
+    } else {
+        ok = kt == JT_STR;   // a string with escapes is still a str: the host decodes it
+        if (kt != JT_STR && kt != JT_ESC && kt != JT_NONE) flags |= DAMPR_TF_JSON_KEY_KIND;
+    }
+    if (tab.val_field != DAMPR_FIELD_VAL_ONE) {
+        const u32 vt = (mt >> (4 * tab.val_field)) & 0xFu;
+        const u32 vb = member_bounds<JM>(mb, tab.val_field);
+        const u8 *vp = t + (vb & 0xFFFFu);
+        const u32 vlen = (vb >> 16) - (vb & 0xFFFFu);
+        if constexpr (VK == VK_F64) {
+            double d;
+            long long iv;
+            if (vt != JT_FLOAT && vt != JT_NONE) flags |= DAMPR_TF_JSON_VAL_KIND;
+            if (vt == JT_INT && parse_int(vp, vlen, iv)) val = __double_as_longlong((double)iv);   // float(-0) is 0.0
+            else if ((vt == JT_INT || vt == JT_FLOAT) && parse_f64(vp, vlen, d)) val = __double_as_longlong(d);
+            else ok = false;
+        } else {
+            if (vt != JT_INT && vt != JT_NONE) flags |= DAMPR_TF_JSON_VAL_KIND;
+            if (!(vt == JT_INT && parse_int(vp, vlen, val))) ok = false;
+        }
+    }
+    if (!ok) {
+        to_host = true;
+        return;
+    }
+    if (!tab.key_int) {
+        if (klen >= 1 && klen <= 9) {
+            for (int i = (int)klen - 1; i >= 0; --i) code = (code << 7) | t[ks + i];
+        } else {
+            code = hash_bytes(t + ks, klen, tab.seed);
+            rep = ((g0 + ks) << 20) | klen;
+            acc_long++;
+        }
+    }
+}
+
 // the kernel body over the tiles of [own_lo, own_hi); where: the predicates of a WHERE scan; WS: split on runs of
-// whitespace (`line.split()`) instead of the separator byte
-template <int VK, int MODE, bool WHERE, bool WS>
+// whitespace (`line.split()`) instead of the separator byte; JSON: json.loads each line and read the members *json
+template <int VK, int MODE, bool WHERE, bool WS, bool JSON = false>
 __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi,
-                                             const FieldsView &tab, const RecView &rv, const WhereView *where) {
+                                             const FieldsView &tab, const RecView &rv, const WhereView *where,
+                                             const JsonView *json = nullptr) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SmemF &s = *reinterpret_cast<SmemF *>(smem_raw);
     const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -449,7 +741,10 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
             bool dropped = false;   // WHERE: a predicate is false
             long long val = 1, kval = 0;
             u64 code = 0, rep = ~0ULL;
-            if (!to_host) {
+            if constexpr (JSON) {
+                if (!to_host) json_fold<VK, WHERE>(s.text, q, end, gq - q, tab, *json, where, to_host, dropped, val, code,
+                                                   rep, acc_long, my_flags);
+            } else if (!to_host) {
                 // resolve the field indices (Python semantics: negative counts from the end)
                 const int nf = WS ? (int)nsep : (int)nsep + 1;
                 const int ki = tab.key_field < 0 ? tab.key_field + nf : tab.key_field;
@@ -680,16 +975,44 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
     fields_tiles<VK, MODE, true, WS>(text, n, own_lo, own_hi, tab, rv, &where);
 }
 
+// the JSON-lines builds: the member names (and a WHERE scan's predicates) read in place from the parameters. The
+// launch runs 4 CTAs per SM; saying so keeps ptxas from squeezing the plain build into 32 registers and spilling.
+template <int VK, int MODE>
+__global__ void __launch_bounds__(F_THREADS, 4)
+text_json_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv,
+                        const __grid_constant__ JsonView json) {
+    fields_tiles<VK, MODE, false, false, true>(text, n, own_lo, own_hi, tab, rv, nullptr, &json);
+}
+
+template <int VK, int MODE>
+__global__ void __launch_bounds__(F_THREADS, 4)
+text_json_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv,
+                        const __grid_constant__ JsonView json, const __grid_constant__ WhereView where) {
+    fields_tiles<VK, MODE, true, false, true>(text, n, own_lo, own_hi, tab, rv, &where, &json);
+}
+static_assert(sizeof(WhereView) + sizeof(JsonView) + 256 <= 4096, "kernel parameters");
+
 // one kernel over the tiles of [own_lo, own_hi); WHERE: the build that applies the predicates *wh; WS: the
-// whitespace-split build
-template <int VK, int MODE, bool WHERE = false, bool WS = false>
+// whitespace-split build; JSON: the JSON-lines build over the members *jv
+template <int VK, int MODE, bool WHERE = false, bool WS = false, bool JSON = false>
 int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const FieldsView &tv, const RecView &rv,
-                  int timer, const WhereView *wh = nullptr) {
+                  int timer, const WhereView *wh = nullptr, const JsonView *jv = nullptr) {
     const size_t smem = sizeof(SmemF);
     const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
     u64 grid = (u64)ctx->num_sms * 4;
     if (grid > ntiles) grid = ntiles;
-    if constexpr (WHERE) {
+    if constexpr (JSON && WHERE) {
+        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonView, WhereView) =
+            text_json_fields_kernel<VK, MODE>;
+        CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ScopedTimer tm(ctx, timer);
+        kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *jv, *wh);
+    } else if constexpr (JSON) {
+        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonView) = text_json_fields_kernel<VK, MODE>;
+        CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ScopedTimer tm(ctx, timer);
+        kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *jv);
+    } else if constexpr (WHERE) {
         void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, WhereView) =
             text_fields_kernel<VK, MODE, true, WS>;
         CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -706,7 +1029,8 @@ int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, con
 }
 
 // the predicates of spec in kernel-parameter form; DAMPR_ERR_ARG for a kind, comparison or limit outside the header's
-int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, WhereView &w) {
+// (json: the predicates of a JSON scan, whose fields index the nmembers members; DAMPR_PRED_MEMBER instead of NFIELDS)
+int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, WhereView &w, bool json = false, int nmembers = 0) {
     ARG_CHECK(ctx, spec->npreds >= 0 && spec->npreds <= DAMPR_PRED_MAX, "npreds must be 0 .. DAMPR_PRED_MAX");
     ARG_CHECK(ctx, spec->npreds == 0 || spec->preds != nullptr, "null preds");
     w = WhereView{};
@@ -715,10 +1039,20 @@ int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, WhereView &w) {
     for (int j = 0; j < spec->npreds; ++j) {
         const dampr_field_pred &p = spec->preds[j];
         const bool in = p.cmp == DAMPR_CMP_IN || p.cmp == DAMPR_CMP_NOT_IN;
-        ARG_CHECK(ctx, p.kind >= DAMPR_PRED_STR && p.kind <= DAMPR_PRED_NFIELDS, "predicate kind");
+        const bool member = json && p.kind == DAMPR_PRED_MEMBER;
+        if (json) {
+            ARG_CHECK(ctx, p.kind >= DAMPR_PRED_STR && p.kind <= DAMPR_PRED_MEMBER && p.kind != DAMPR_PRED_NFIELDS,
+                      "predicate kind of a JSON scan");
+            ARG_CHECK(ctx, p.field >= 0 && p.field < nmembers, "a JSON predicate's field must index the members");
+        } else {
+            ARG_CHECK(ctx, p.kind >= DAMPR_PRED_STR && p.kind <= DAMPR_PRED_NFIELDS, "predicate kind");
+        }
         ARG_CHECK(ctx, p.cmp >= DAMPR_CMP_EQ && p.cmp <= DAMPR_CMP_NOT_IN, "predicate comparison");
-        ARG_CHECK(ctx, !in || p.kind == DAMPR_PRED_STR || p.kind == DAMPR_PRED_INT, "IN / NOT_IN take STR or INT");
-        ARG_CHECK(ctx, in ? (p.n >= 1 && p.n <= DAMPR_PRED_MAX_CONSTS) : p.n == 1, "predicate constant count");
+        ARG_CHECK(ctx, !member || in, "DAMPR_PRED_MEMBER takes IN or NOT_IN");
+        ARG_CHECK(ctx, !in || member || p.kind == DAMPR_PRED_STR || p.kind == DAMPR_PRED_INT,
+                  "IN / NOT_IN take STR or INT");
+        ARG_CHECK(ctx, member ? p.n == 0 : in ? (p.n >= 1 && p.n <= DAMPR_PRED_MAX_CONSTS) : p.n == 1,
+                  "predicate constant count");
         ARG_CHECK(ctx, nc + p.n <= DAMPR_PRED_MAX_CONSTS, "more than DAMPR_PRED_MAX_CONSTS predicate constants");
         w.p[j] = PredSlot{p.field, (u8)p.kind, (u8)p.cmp, (u8)nc, (u8)p.n};
         for (int i = 0; i < p.n; ++i, ++nc) {
@@ -757,6 +1091,37 @@ int check_fields_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own
     return where_view(ctx, spec, w);
 }
 
+// the arguments of a JSON call and its member names in kernel-parameter form
+int check_json_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own_lo, u64 own_hi,
+                    const dampr_fields_spec *spec, const dampr_json_members *m, JsonView &jv) {
+    ARG_CHECK(ctx, ctx && t && tb && spec && m, "null");
+    ARG_CHECK(ctx, own_lo <= own_hi && own_hi <= tb->n, "ownership range outside the text");
+    ARG_CHECK(ctx, (own_lo % 16) == 0, "own_lo must be a multiple of 16");
+    ARG_CHECK(ctx, spec->sep == DAMPR_FIELD_SEP_JSON, "a JSON call takes sep DAMPR_FIELD_SEP_JSON");
+    ARG_CHECK(ctx, spec->key_kind == DAMPR_FIELD_KEY_STR || spec->key_kind == DAMPR_FIELD_KEY_INT, "key kind");
+    ARG_CHECK(ctx, m->n >= 1 && m->n <= J_MAX, "1 .. DAMPR_JSON_MAX_MEMBERS members");
+    ARG_CHECK(ctx, m->len != nullptr && m->bytes != nullptr, "null member names");
+    ARG_CHECK(ctx, spec->key_field >= 0 && spec->key_field < m->n, "key_field must index the members");
+    ARG_CHECK(ctx, spec->val_field == DAMPR_FIELD_VAL_ONE || (spec->val_field >= 0 && spec->val_field < m->n),
+              "val_field must index the members or be DAMPR_FIELD_VAL_ONE");
+    jv = JsonView{};
+    jv.n = m->n;
+    int off = 0;
+    for (int j = 0; j < m->n; ++j) {
+        ARG_CHECK(ctx, m->len[j] >= 0 && m->len[j] <= J_NAME, "a member name of 0 .. DAMPR_JSON_MAX_NAME bytes");
+        for (int i = 0; i < m->len[j]; ++i) {
+            const u8 c = (u8)m->bytes[off + i];
+            ARG_CHECK(ctx, c >= 0x20 && c < 0x80 && c != '"' && c != '\\',
+                      "member names are ASCII without '\"', '\\\\' or bytes below 0x20");
+            jv.name[j][i] = c;
+        }
+        jv.len[j] = (u8)m->len[j];
+        off += m->len[j];
+    }
+    WhereView w;
+    return where_view(ctx, spec, w, true, m->n);
+}
+
 FieldsView fields_view(dampr_table *t, const dampr_fields_spec *spec, int op) {
     return FieldsView{t->keys, t->counts, t->reps, t->stats, t->fb, t->cap - 1, 0x243F6A8885A308D3ULL, t->fb_cap,
                       (u32)spec->sep, spec->key_field, spec->val_field, spec->key_kind == DAMPR_FIELD_KEY_INT ? 1 : 0,
@@ -775,12 +1140,49 @@ int launch_fold_sep(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, c
     return launch_fields<VK, MODE, true, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w);
 }
 
+// the fold pass of one range of a JSON scan: the plain build reads two members, the WHERE build (also taken without
+// predicates when more members are listed) up to J_MAX
+template <int VK, int MODE>
+int launch_json_fold(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
+                     const JsonView &jv, const FieldsView &tv, const RecView &rv) {
+    if (spec->npreds == 0 && jv.n <= 2)
+        return launch_fields<VK, MODE, false, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS,
+                                                          nullptr, &jv);
+    WhereView w;
+    if (int r = where_view(ctx, spec, w, true, jv.n)) return r;
+    return launch_fields<VK, MODE, true, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w, &jv);
+}
+
 // the fold pass of one range: the separator-byte build, or the whitespace-split one under DAMPR_FIELD_SEP_WS
 template <int VK, int MODE>
 int launch_fold(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
                 const FieldsView &tv, const RecView &rv) {
     if (spec->sep == DAMPR_FIELD_SEP_WS) return launch_fold_sep<VK, MODE, true>(ctx, tb, own_lo, own_hi, spec, tv, rv);
     return launch_fold_sep<VK, MODE, false>(ctx, tb, own_lo, own_hi, spec, tv, rv);
+}
+
+// record mode's first two kernels over one range: lines per tile (the tile array grown to the range), then the
+// tile bases scanned from the running record count
+int count_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const FieldsView &tv,
+                  RecView &rv) {
+    const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
+    if (ntiles > t->tiles_cap) {
+        CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));   // the previous range may still read the old array
+        cudaFree(t->tiles);
+        t->tiles = nullptr;
+        t->tiles_cap = 0;
+        CUDA_TRY(ctx, cudaMalloc(&t->tiles, ntiles * sizeof(u64)));
+        t->tiles_cap = ntiles;
+    }
+    rv.tiles = t->tiles;
+    wait_uploads(ctx);
+    if (int r = launch_fields<VK_INT, M_COUNT>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS_COUNT)) return r;
+    {
+        ScopedTimer tm(ctx, DAMPR_K_TEXT_FIELDS_COUNT);
+        fields_tile_scan_kernel<<<1, SCAN_THREADS, 0, ctx->stream>>>(t->tiles, ntiles, t->stats + S_RECORDS);
+    }
+    CUDA_TRY(ctx, cudaGetLastError());
+    return DAMPR_OK;
 }
 
 }  // namespace
@@ -808,24 +1210,44 @@ extern "C" int32_t dampr_text_fields_records(dampr_ctx *ctx, dampr_table *t, dam
               "op must be DAMPR_OP_SUM_I64 or DAMPR_OP_SUM_F64");
     ARG_CHECK(ctx, spec->val_field != DAMPR_FIELD_VAL_ONE, "record mode needs a value field");
     if (own_hi <= own_lo) return DAMPR_OK;
-    const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
-    if (ntiles > t->tiles_cap) {
-        CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));   // the previous range may still read the old array
-        cudaFree(t->tiles);
-        t->tiles = nullptr;
-        t->tiles_cap = 0;
-        CUDA_TRY(ctx, cudaMalloc(&t->tiles, ntiles * sizeof(u64)));
-        t->tiles_cap = ntiles;
-    }
     const FieldsView tv = fields_view(t, spec, DAMPR_OP_SUM_I64);   // the table counts the lines of each key
-    const RecView rv{rec->rec, rec->capacity, t->tiles};
-    wait_uploads(ctx);
-    if (int r = launch_fields<VK_INT, M_COUNT>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS_COUNT)) return r;
-    {
-        ScopedTimer tm(ctx, DAMPR_K_TEXT_FIELDS_COUNT);
-        fields_tile_scan_kernel<<<1, SCAN_THREADS, 0, ctx->stream>>>(t->tiles, ntiles, t->stats + S_RECORDS);
-    }
-    CUDA_TRY(ctx, cudaGetLastError());
+    RecView rv{rec->rec, rec->capacity, nullptr};
+    if (int r = count_records(ctx, t, tb, own_lo, own_hi, tv, rv)) return r;
     if (spec->op == DAMPR_OP_SUM_F64) return launch_fold<VK_F64, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, tv, rv);
     return launch_fold<VK_INT, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, tv, rv);
+}
+
+extern "C" int32_t dampr_text_json_fields(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
+                                          uint64_t own_hi, const dampr_fields_spec *spec,
+                                          const dampr_json_members *members) {
+    JsonView jv;
+    if (int r = check_json_args(ctx, t, tb, own_lo, own_hi, spec, members, jv)) return r;
+    const bool f64 = spec->op == DAMPR_OP_MIN_F64 || spec->op == DAMPR_OP_MAX_F64;
+    ARG_CHECK(ctx, f64 || spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_MIN_I64 ||
+                       spec->op == DAMPR_OP_MAX_I64,
+              "op must be DAMPR_OP_SUM_I64, DAMPR_OP_MIN_I64, DAMPR_OP_MAX_I64, DAMPR_OP_MIN_F64 or DAMPR_OP_MAX_F64");
+    ARG_CHECK(ctx, !f64 || spec->val_field != DAMPR_FIELD_VAL_ONE, "a float op needs a value field");
+    if (own_hi <= own_lo) return DAMPR_OK;
+    const FieldsView tv = fields_view(t, spec, spec->op);
+    wait_uploads(ctx);
+    if (f64) return launch_json_fold<VK_F64, M_TABLE>(ctx, tb, own_lo, own_hi, spec, jv, tv, RecView{});
+    return launch_json_fold<VK_INT, M_TABLE>(ctx, tb, own_lo, own_hi, spec, jv, tv, RecView{});
+}
+
+extern "C" int32_t dampr_text_json_fields_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb,
+                                                  uint64_t own_lo, uint64_t own_hi, const dampr_fields_spec *spec,
+                                                  const dampr_json_members *members, dampr_kv *rec) {
+    JsonView jv;
+    if (int r = check_json_args(ctx, t, tb, own_lo, own_hi, spec, members, jv)) return r;
+    ARG_CHECK(ctx, rec != nullptr, "null");
+    ARG_CHECK(ctx, spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_SUM_F64,
+              "op must be DAMPR_OP_SUM_I64 or DAMPR_OP_SUM_F64");
+    ARG_CHECK(ctx, spec->val_field != DAMPR_FIELD_VAL_ONE, "record mode needs a value field");
+    if (own_hi <= own_lo) return DAMPR_OK;
+    const FieldsView tv = fields_view(t, spec, DAMPR_OP_SUM_I64);
+    RecView rv{rec->rec, rec->capacity, nullptr};
+    if (int r = count_records(ctx, t, tb, own_lo, own_hi, tv, rv)) return r;
+    if (spec->op == DAMPR_OP_SUM_F64)
+        return launch_json_fold<VK_F64, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, jv, tv, rv);
+    return launch_json_fold<VK_INT, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, jv, tv, rv);
 }

@@ -27,14 +27,17 @@ OP_SUM_I64, OP_SUM_F64, OP_COUNT, OP_MIN_I64, OP_MAX_I64, OP_MIN_F64, OP_MAX_F64
 # table flags
 TF_NONASCII, TF_CR, TF_LONGLINE, TF_TABLEFULL, TF_LONGTOKEN, TF_COLLISION = 1, 2, 4, 8, 16, 32
 TF_RECFULL, TF_NEGZERO = 64, 128   # field scans: record buffer full / a float() field parsed to -0.0
+TF_JSON_KEY_KIND, TF_JSON_VAL_KIND = 256, 512   # JSON scans: a key / value member of the other JSON kind
 TOK_FLAG_CR_DATA = 0x100
 # delimited-field scans (dampr_text_fields)
 FIELD_KEY_STR, FIELD_KEY_INT = 0, 1
 FIELD_VAL_ONE = 0x7FFFFFFF
 FIELD_SEP_WS = 256   # sep: split like str.split() (runs of ASCII whitespace, no '' fields)
+FIELD_SEP_JSON = 257   # sep of the JSON-lines calls: fields are the members of json.loads(line)
+JSON_MAX_MEMBERS, JSON_MAX_NAME, JSON_MAX_DEPTH = 8, 64, 64
 FIELDS_HALO = 65536
 # WHERE predicates of a field scan (dampr_field_pred): kinds, comparisons, limits per call
-PRED_STR, PRED_INT, PRED_F64, PRED_NFIELDS = range(4)
+PRED_STR, PRED_INT, PRED_F64, PRED_NFIELDS, PRED_MEMBER = range(5)
 CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_IN, CMP_NOT_IN = range(8)
 PRED_MAX, PRED_MAX_CONSTS, PRED_MAX_BYTES = 8, 64, 1024
 
@@ -99,6 +102,20 @@ def fields_spec(spec, cr_is_data, preds):
     return s
 
 
+class JsonMembers(C.Structure):
+    """dampr_json_members"""
+    _fields_ = [("n", C.c_int32), ("bytes", C.c_char_p), ("len", C.POINTER(C.c_int32))]
+
+
+def json_members(names):
+    """dampr_json_members of the member names (str); the returned structure keeps its arrays alive"""
+    raw = [n.encode("ascii") for n in names]
+    ln = (C.c_int32 * max(1, len(raw)))(*map(len, raw))
+    m = JsonMembers(len(raw), b"".join(raw), C.cast(ln, C.POINTER(C.c_int32)))
+    m._keep = ln
+    return m
+
+
 class DeviceError(RuntimeError):
     pass
 
@@ -159,6 +176,9 @@ def load_library():
     _sig(lib, "dampr_text_verify", vp, vp, vp, u64, u64, i32)
     _sig(lib, "dampr_text_fields", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec))
     _sig(lib, "dampr_text_fields_records", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), vp)
+    _sig(lib, "dampr_text_json_fields", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), C.POINTER(JsonMembers))
+    _sig(lib, "dampr_text_json_fields_records", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), C.POINTER(JsonMembers),
+         vp)
     _sig(lib, "dampr_table_stats", vp, vp, pu64)
     _sig(lib, "dampr_table_fallback_lines", vp, vp, vp, u64, pu64)
     _sig(lib, "dampr_table_fetch", vp, vp, vp, vp, vp, u64, pu64)
@@ -595,6 +615,19 @@ class Table(object):
         s = fields_spec(spec, cr_is_data, preds)
         self.ctx.check(self.ctx.lib.dampr_text_fields_records(self.ctx.h, self.h, tb.h, int(lo), int(hi), C.byref(s),
                                                               kv.h))
+
+    def json_fields(self, tb, lo, hi, spec, members, cr_is_data=False, preds=()):
+        """fields() over JSON lines: spec = (FIELD_SEP_JSON, key member, key kind, value member or FIELD_VAL_ONE, op),
+        the member indices (and the predicates' fields) index `members`, a list of member names"""
+        s, m = fields_spec(spec, cr_is_data, preds), json_members(members)
+        self.ctx.check(self.ctx.lib.dampr_text_json_fields(self.ctx.h, self.h, tb.h, int(lo), int(hi), C.byref(s),
+                                                           C.byref(m)))
+
+    def json_fields_records(self, tb, lo, hi, spec, members, kv, cr_is_data=False, preds=()):
+        """fields_records() over JSON lines, spec and members as json_fields()"""
+        s, m = fields_spec(spec, cr_is_data, preds), json_members(members)
+        self.ctx.check(self.ctx.lib.dampr_text_json_fields_records(self.ctx.h, self.h, tb.h, int(lo), int(hi),
+                                                                   C.byref(s), C.byref(m), kv.h))
 
     def fields_stats(self):
         """stats() of a field scan under the names of its counters. "records" is the record count in record mode;

@@ -414,6 +414,135 @@ def field_predicate(fn, record=None, whitespace=False):
     return sep, kind, i, op, consts
 
 
+# ---- JSON lines: Dampr.json(path) = map(json.loads) in front of the fold ----------------------------------------
+FIELD_DATA = "data"       # a bare r["m"]: its Python type is the JSON value's, decided by the data
+FIELD_MEMBER = "member"   # "m" in r / "m" not in r
+
+
+def is_json_loads(fn):
+    """True for json.loads itself (Dampr.json's mapper) and for `lambda l: json.loads(l)`"""
+    import json
+    if fn is json.loads:
+        return True
+    if not (isinstance(fn, types.FunctionType) and fn.__code__.co_argcount == 1):
+        return False
+    e = analyze(fn)
+    if e is None or e.op != "call" or len(e.b) != 1 or not _is_arg(e.b[0]) or not isinstance(e.a, E):
+        return False
+    f = e.a
+    if f.op == "attr" and isinstance(f.a, E) and f.a.op == "obj":   # json.loads(l)
+        return getattr(f.a.a, f.b, None) is json.loads
+    return f.op == "obj" and f.a is json.loads                      # loads(l) after `from json import loads`
+
+
+def json_member_name(name):
+    """True if the device matches member `name` by its bytes: ASCII, at most 64 bytes, no '"', '\\' or control
+    character (a JSON line spells every other name with an escape, or cannot hold it)"""
+    return type(name) is str and len(name) <= 64 and all(0x20 <= ord(c) < 0x80 for c in name) and \
+        '"' not in name and "\\" not in name
+
+
+def _member(e):
+    """(kind, name) if e is r["m"] (FIELD_DATA), int(r["m"]) (FIELD_INT) or float(r["m"]) (FIELD_FLOAT) over the
+    argument r with a constant name the device matches, else None"""
+    kind = FIELD_DATA
+    if isinstance(e, E) and e.op == "call" and isinstance(e.a, E) and e.a.op == "obj" and e.a.a in (int, float) \
+            and len(e.b) == 1:
+        kind, e = FIELD_INT if e.a.a is int else FIELD_FLOAT, e.b[0]
+    if not (isinstance(e, E) and e.op == "sub" and _is_arg(e.a)):
+        return None
+    ok, name = _const(e.b)
+    return (kind, name) if ok and json_member_name(name) else None
+
+
+def json_fields_spec(key_fn, value_fn):
+    """Device JSON-lines spec of a keyed(key_fn, value_fn) behind map(json.loads): (key name, key kind, value name,
+    value kind, mean) where the key is r["k"] (FIELD_DATA) or int(r["k"]) (FIELD_INT), and the value is
+      the constant 1                                        value name None, FIELD_INT, mean False
+      r["v"] (FIELD_DATA), int(r["v"]) or float(r["v"])     mean False
+      mean()'s `(value(r), 1)`, value one of those          mean True
+    None for any other shape (r.get, r["a"]["b"], tuple keys, float keys, ...)."""
+    fns = (key_fn, value_fn)
+    if not all(isinstance(f, types.FunctionType) and f.__code__.co_argcount == 1 for f in fns):
+        return None
+    ke, ve = analyze(key_fn), analyze(value_fn)
+    if ke is None or ve is None:
+        return None
+    k = _member(ke)
+    if k is None or k[0] == FIELD_FLOAT:
+        return None
+    if _is_one(ve):
+        return k[1], k[0], None, FIELD_INT, False
+    mean = ve.op == "tuple" and len(ve.a) == 2
+    if mean:
+        inner = _inline_call_of_arg(ve.a[0])
+        if inner is None or not _is_one(ve.a[1]):
+            return None
+        ve = inner
+    v = _member(ve)
+    if v is None:
+        return None
+    return k[1], k[0], v[1], v[0], mean
+
+
+def json_predicate(fn):
+    """Device WHERE predicate of a `filter(fn)` behind map(json.loads), or None. Returns (kind, name, op, constants):
+      "m" in r, "m" not in r   kind FIELD_MEMBER, constants ()
+      M op C, C op M           M = r["m"] with C a str (kind FIELD_STR) or an int in int64, not a bool (FIELD_INT);
+                               M = int(r["m"]) with C such an int (FIELD_INT); M = float(r["m"]) with C a float or an
+                               int with |C| <= 2^53 (FIELD_FLOAT, C returned as a float); op one of == != < <= > >=
+      M in K, M not in K       M = r["m"] or int(r["m"]); K a tuple / frozenset / set / list (literal, closure or
+                               global) of 1 .. PRED_MAX_CONSTS members, all str (r["m"] only) or all int in int64
+    A bare r["m"] against a float constant, and everything field_predicate refuses, is None."""
+    if not (isinstance(fn, types.FunctionType) and fn.__code__.co_argcount == 1):
+        return None
+    e = analyze(fn)
+    if e is None or e.op != "cmp":
+        return None
+    op, l, r = e.a, e.b, e.c
+    if op in ("in", "not in") and _is_arg(r):
+        ok, name = _const(l)
+        return (FIELD_MEMBER, name, op, ()) if ok and json_member_name(name) else None
+    if op in _FLIP and _pred_const(l)[0] and not _pred_const(r)[0]:
+        op, l, r = _FLIP[op], r, l
+    ok, c = _pred_const(r)
+    m = _member(l)
+    if not ok or m is None:
+        return None
+    kind, name = m
+    if op in ("in", "not in"):
+        if kind == FIELD_FLOAT or type(c) not in (tuple, frozenset, set, list) or not 1 <= len(c) <= PRED_MAX_CONSTS:
+            return None
+        consts = tuple(c)
+    elif op in _FLIP:
+        consts = (c,)
+    else:
+        return None
+    if kind == FIELD_DATA:
+        if all(type(x) is str for x in consts):
+            kind = FIELD_STR
+        elif all(type(x) is int for x in consts):
+            kind = FIELD_INT
+        else:
+            return None
+    if kind == FIELD_STR:
+        try:
+            if sum(len(x.encode("utf-8")) for x in consts) > PRED_MAX_BYTES:
+                return None
+        except UnicodeEncodeError:   # a lone surrogate: no UTF-8 bytes to compare
+            return None
+    elif kind == FIELD_INT:
+        if not all(type(x) is int and -(1 << 63) <= x < (1 << 63) for x in consts):
+            return None
+    else:
+        v = consts[0]
+        if type(v) is int and abs(v) <= (1 << 53):
+            consts = (float(v),)
+        elif type(v) is not float:
+            return None
+    return kind, name, op, consts
+
+
 def field_index(fn):
     """i if fn is `lambda x: x[i]` with a constant non-negative int i, else None."""
     e = analyze(fn)

@@ -807,6 +807,8 @@ class FieldScan(TextScan):
         flags = st["flags"]
         if self._grow_table(tab, st):
             return self._run()
+        if self._kind_retry(st):
+            return self._run()
         if flags & dev.TF_TABLEFULL:
             raise NotLowerable("combiner table overflow")
         if flags & (dev.TF_NONASCII | dev.TF_LONGLINE):
@@ -837,6 +839,7 @@ class FieldScan(TextScan):
                 it = p.stream(it)
             for k, v in it:
                 nrec += 1
+                self._check_host_kinds(k, v)
                 if not self.float_values:
                     max_abs = max(max_abs, abs(v[0] if self.mean else v))
                 elif self.op != dev.OP_SUM_F64 and (v != v or (v == 0 and math.copysign(1.0, v) < 0)):
@@ -860,6 +863,13 @@ class FieldScan(TextScan):
         if self.preds:   # the table-mode slot, or the records that are neither folded nor handed back
             self.filtered = int(st["records"]) - (int(st["lines"]) + int(st["fallback"]) if self.records else 0)
         return self
+
+    def _kind_retry(self, st):
+        """True when the scan is to be repeated with other key or value kinds (JSON scans)"""
+        return False
+
+    def _check_host_kinds(self, k, v):
+        """raise NotLowerable when a host line's key or value would give the device's column another type"""
 
     def _record_sums(self, codes, n):
         """per table key code (in `codes` order): the sum of its records' values, folded in line order by the stable
@@ -888,6 +898,72 @@ class FieldScan(TextScan):
         if len(codes) != len(rk) or (len(codes) and not np.array_equal(rk[np.minimum(pos, len(rk) - 1)], codes)):
             raise NotLowerable("field records and table keys disagree")
         return rv[pos].view(np.float64 if self.op == dev.OP_SUM_F64 else np.int64)
+
+
+class JsonFieldScan(FieldScan):
+    """FieldScan over JSON lines (dampr_text_json_fields): the members of json.loads(line) instead of split fields.
+
+    A bare r["k"] or r["v"] gives whatever Python type the JSON value has. The scan starts with str keys and int values;
+    when the device took no line and saw only the other kind (DAMPR_TF_JSON_KEY_KIND / DAMPR_TF_JSON_VAL_KIND), it is
+    repeated once with int keys or float values. A bare member of mixed kinds, or a host line whose bare key or value
+    has another type than the device's column, sends the stage to the host map."""
+
+    _FLOAT_OPS = {dev.OP_SUM_I64: dev.OP_SUM_F64, dev.OP_MIN_I64: dev.OP_MIN_F64, dev.OP_MAX_I64: dev.OP_MAX_F64}
+
+    def __init__(self, runner, sources, spec, op, stage, mean, preds, members, bare):
+        FieldScan.__init__(self, runner, sources, spec, op, stage, mean, preds)
+        self.members = members              # the member names the spec and the predicates index
+        self.bare_key, self.bare_val = bare
+        self._kinds_retried = False
+
+    def _launch(self, tab, tb, lo, hi):
+        spec = tuple(self.spec) + (self.op,)
+        cr = getattr(self, "_cr_is_data", False)
+        if not self.records:
+            tab.json_fields(tb, lo, hi, spec, self.members, cr, self.preds)
+            return
+        if self._rec is None:
+            self._records_buffer(min(tb.n // 32 + 4096, self._free_bytes() // (2 * self.REC_BYTES)))
+        tab.json_fields_records(tb, lo, hi, spec, self.members, self._rec, cr, self.preds)
+
+    def _fallback_lines(self, tb, tab):
+        """the host lines in offset order, a blank one included: it is the empty line json.loads('') raises on (the
+        reader's split of a zero-length piece yields no line)"""
+        blank = sorted(e >> 16 for e in tab.fallback_lines().tolist() if e & 0xFFFF == 0)
+        i = 0
+        for off, line in FieldScan._fallback_lines(self, tb, tab):
+            while i < len(blank) and blank[i] < off:
+                yield blank[i], ""
+                i += 1
+            yield off, line
+        for off in blank[i:]:
+            yield off, ""
+
+    def _kind_retry(self, st):
+        key = self.bare_key and st["flags"] & dev.TF_JSON_KEY_KIND
+        val = self.bare_val and st["flags"] & dev.TF_JSON_VAL_KIND
+        if not (key or val):
+            return False
+        if self._kinds_retried or st["lines"]:
+            raise NotLowerable("a bare JSON member of more than one kind")
+        self._kinds_retried = True
+        sep, ki, kkind, vi = self.spec
+        if key:
+            kkind = dev.FIELD_KEY_INT
+        if val:
+            self.op = self._FLOAT_OPS[self.op]
+            self.records = self.mean or self.op == dev.OP_SUM_F64
+            self.float_values = True
+        self.spec = (sep, ki, kkind, vi)
+        self._free_records()
+        self._rec_regrown = False
+        return True
+
+    def _check_host_kinds(self, k, v):
+        if self.bare_key and type(k) is not (int if self.spec[2] == dev.FIELD_KEY_INT else str):
+            raise NotLowerable("a host line's JSON key has another type than the device's keys")
+        if self.bare_val and type(v[0] if self.mean else v) is not (float if self.float_values else int):
+            raise NotLowerable("a host line's JSON value has another type than the device's values")
 
 
 def _key_positions(keys, extra):
@@ -1066,6 +1142,63 @@ def _match_text_fields(stage, inputs):
                  dev.FIELD_VAL_ONE if vi is None else vi), op, mean, tuple(preds)
 
 
+def _match_json_fields(stage, inputs):
+    """map(json.loads) filter* keyed(r["k"] | int(r["k"]), 1 | r["v"] | int(r["v"]) | float(r["v"])) +
+    PartialReduceCombiner(+ | min | max), or mean()'s keyed(key, (value, 1)) + component-wise (+, +), over text, each
+    filter one lowering.json_predicate: (sources, (FIELD_SEP_JSON, key member, key kind, value member or FIELD_VAL_ONE),
+    op, mean, device predicates, member names, (bare key, bare value)) or None"""
+    if not isinstance(stage, GMap) or len(inputs) != 1:
+        return None
+    src = _text_files(inputs[0])
+    if src is None:
+        return None
+    ks = _opkinds(stage.mapper)
+    kinds = [k for k, _ in ks] if ks is not None else []
+    if len(kinds) < 2 or kinds[0] != "map" or kinds[-1] != "keyed" or any(k != "filter" for k in kinds[1:-1]):
+        return None
+    if not lowering.is_json_loads(ks[0][1].fn) or not isinstance(stage.combiner, ops.PartialReduceCombiner):
+        return None
+    keyed = ks[-1][1]
+    spec = lowering.json_fields_spec(keyed.fn, keyed.fn2)
+    if spec is None:
+        return None
+    kname, kkind, vname, vkind, mean = spec
+    members = []
+
+    def member(name):
+        if name not in members:
+            members.append(name)
+        return members.index(name)
+
+    ki = member(kname)
+    vi = dev.FIELD_VAL_ONE if vname is None else member(vname)
+    preds = []
+    for _k, o in ks[1:-1]:
+        p = lowering.json_predicate(o.fn)
+        if p is None:
+            return None
+        kind, name, cmp, consts = p
+        preds.append((dev.PRED_MEMBER if kind == lowering.FIELD_MEMBER else _PRED_KINDS[kind], member(name),
+                      _PRED_CMPS[cmp], consts))
+    if len(members) > dev.JSON_MAX_MEMBERS or len(preds) > dev.PRED_MAX or \
+            sum(len(p[3]) for p in preds) > dev.PRED_MAX_CONSTS or \
+            sum(len(c.encode("utf-8")) for p in preds if p[0] == dev.PRED_STR for c in p[3]) > dev.PRED_MAX_BYTES:
+        return None
+    binop = stage.options.get("binop")
+    if mean:
+        if lowering.tuple_binop_kinds(binop) != [lowering.ADD, lowering.ADD]:
+            return None
+        op = dev.OP_SUM_F64 if vkind == lowering.FIELD_FLOAT else dev.OP_SUM_I64
+    else:
+        kind = lowering.binop_kind(binop)
+        if kind not in (lowering.ADD, lowering.MIN, lowering.MAX):
+            return None
+        op = (_FOLD_OPS_F64 if vkind == lowering.FIELD_FLOAT else _FOLD_OPS)[kind]
+    return src, (dev.FIELD_SEP_JSON, ki, dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR,
+                 vi), op, mean, tuple(preds), tuple(members), \
+        (kkind == lowering.FIELD_DATA, vkind == lowering.FIELD_DATA)
+
+
 _PRED_KINDS = {lowering.FIELD_STR: dev.PRED_STR, lowering.FIELD_INT: dev.PRED_INT, lowering.FIELD_FLOAT: dev.PRED_F64,
                lowering.FIELD_COUNT: dev.PRED_NFIELDS}
 _PRED_CMPS = {"==": dev.CMP_EQ, "!=": dev.CMP_NE, "<": dev.CMP_LT, "<=": dev.CMP_LE, ">": dev.CMP_GT, ">=": dev.CMP_GE,
@@ -1167,6 +1300,21 @@ def _lower_map(runner, stage, inputs, si):
         if spec[0] == dev.FIELD_SEP_WS:
             detail += " sep=ws"
         runner.stats.add(stage, "device text fields scan+combine", detail)
+        return Frame(scan.keys, [scan.values], scalar=True, combined=True)
+    m = _match_json_fields(stage, inputs)
+    if m is not None:
+        if dist.active():
+            raise NotLowerable("the JSON field scan runs on one process")
+        src, spec, op, mean, preds, members, bare = m
+        scan = JsonFieldScan(runner, src, spec, op, stage, mean, preds, members, bare).run()
+        op, spec = scan.op, scan.spec   # after a kind retry
+        opname = ("mean_f64" if op == dev.OP_SUM_F64 else "mean_i64") if mean else \
+            "count" if spec[3] == dev.FIELD_VAL_ONE and op == dev.OP_SUM_I64 else _FIELD_OP_NAMES[op]
+        detail = "op=%s bytes=%d lines=%d groups=%d host_lines=%d" % (opname, scan.nbytes, scan.n_lines, scan.groups,
+                                                                      scan.host_lines)
+        if preds:
+            detail += " filtered=%d" % scan.filtered
+        runner.stats.add(stage, "device text fields scan+combine", detail + " sep=json")
         return Frame(scan.keys, [scan.values], scalar=True, combined=True)
     if _match_line_count(stage, inputs):
         ds = inputs[0]

@@ -164,6 +164,8 @@ int32_t dampr_text_verify(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uin
 #define DAMPR_TF_COLLISION 32u
 #define DAMPR_TF_RECFULL 64u   /* dampr_text_fields_records: more lines than the record buffer holds            */
 #define DAMPR_TF_NEGZERO 128u  /* a float() field scan parsed a negative zero                                    */
+#define DAMPR_TF_JSON_KEY_KIND 256u  /* a JSON scan read a key member of another JSON type than key_kind names       */
+#define DAMPR_TF_JSON_VAL_KIND 512u  /* a JSON scan read a value member of another kind than its fold (see below)     */
 int32_t dampr_table_stats(dampr_ctx *ctx, dampr_table *t, uint64_t stats[8]);
 /* Per-line fallback of the [^\w]+ tokenisers: a line that holds a byte the device cannot tokenise the way
  * Python does (non-ASCII: Unicode \w / lower(); '\r' in text mode: universal newlines) contributes NOTHING to
@@ -195,6 +197,7 @@ int32_t dampr_table_fallback_lines(dampr_ctx *ctx, dampr_table *t, uint64_t *lin
 #define DAMPR_PRED_INT 1      /* int(line.split(sep)[field]) against int64 constants                               */
 #define DAMPR_PRED_F64 2      /* float(line.split(sep)[field]) against one double (IEEE: NaN is unequal to all)    */
 #define DAMPR_PRED_NFIELDS 3  /* len(line.split(sep)) against one int64; `field` is unused                        */
+#define DAMPR_PRED_MEMBER 4   /* JSON scans only: "m" in r (DAMPR_CMP_IN) / "m" not in r (DAMPR_CMP_NOT_IN), n = 0  */
 #define DAMPR_CMP_EQ 0
 #define DAMPR_CMP_NE 1
 #define DAMPR_CMP_LT 2
@@ -270,6 +273,45 @@ int32_t dampr_text_fields(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uin
  * Three kernels per range: a line count per 16 KB tile, one CTA's scan of the counts, the fold. */
 int32_t dampr_text_fields_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
                                   uint64_t own_hi, const dampr_fields_spec *spec, dampr_kv *rec);
+/* ---- JSON-lines fold: `Dampr.json(path)` (map(json.loads)) with r["k"] keys and r["v"] / int(r["v"]) /
+ *      float(r["v"]) values, and filters on r["m"] -------------------------------------------------------------------
+ * The same folds as dampr_text_fields / dampr_text_fields_records with spec->sep = DAMPR_FIELD_SEP_JSON (the field
+ * calls reject it, these calls take nothing else). key_field, val_field and every predicate's `field` index the
+ * member list; no index is negative, and DAMPR_PRED_NFIELDS is not taken. Each line is json.loads'd:
+ * - The device takes a line only when the whole line is one JSON text whose top-level value is an object (json.loads'
+ *   grammar: escapes \" \\ \/ \b \f \n \r \t \uXXXX, no raw byte below 0x20 in a string, numbers
+ *   -?(0|[1-9]\d*)(\.\d+)?([eE][+-]?\d+)?, the literals true / false / null, only JSON whitespace around tokens),
+ *   nested at most DAMPR_JSON_MAX_DEPTH deep, every byte ASCII (no '\r' unless cr_is_data, where it is whitespace),
+ *   no top-level member name holds a backslash, every member it reads exists, and it ends within 4 KB of its start.
+ *   NaN, Infinity and -Infinity are not taken. Every other line is a fallback line, as above.
+ * - Only top-level members count; a name that occurs twice takes its last occurrence (as dict does).
+ * - key_kind STR: the member is a string without escapes, coded like a field key from the bytes between its quotes
+ *   (the representative points at them). INT: a JSON integer of at most 18 digits, coded v ^ 2^63.
+ * - Values: the int ops take a JSON integer of at most 18 digits; the float ops (and DAMPR_OP_SUM_F64 records) take
+ *   any JSON number through the float() rule above.
+ * - A key member of another JSON type than key_kind's (a number, literal, object or array under STR; a string,
+ *   float-syntax number, literal, object or array under INT) sets DAMPR_TF_JSON_KEY_KIND; a value member that is not
+ *   a JSON integer under the int ops, or not a float-syntax number (a '.' or an exponent) under the float ops, sets
+ *   DAMPR_TF_JSON_VAL_KIND. Both only on lines the predicates keep, whatever else the line holds; the line is then a
+ *   fallback line unless the scan takes that member anyway (any number under the float ops). A caller whose r["k"]
+ *   or r["v"] is read bare learns from them that its column would hold another Python type.
+ * - Predicates: STR takes a string member without escapes, INT a JSON integer of at most 18 digits, F64 any JSON
+ *   number; a member of another type, or a missing one, makes the predicate undecided (a fallback line).
+ *   DAMPR_PRED_MEMBER never is. */
+#define DAMPR_FIELD_SEP_JSON 257
+#define DAMPR_JSON_MAX_MEMBERS 8   /* members per call                                                                */
+#define DAMPR_JSON_MAX_NAME 64     /* bytes per member name: ASCII, no '"', '\\' or byte below 0x20                   */
+#define DAMPR_JSON_MAX_DEPTH 64    /* the top-level object is depth 1; a line nested deeper is a fallback line        */
+typedef struct dampr_json_members {
+    int32_t n;               /* 1 .. DAMPR_JSON_MAX_MEMBERS                                                       */
+    const char *bytes;       /* the names back to back                                                             */
+    const int32_t *len;      /* their lengths in bytes                                                             */
+} dampr_json_members;
+int32_t dampr_text_json_fields(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo, uint64_t own_hi,
+                               const dampr_fields_spec *spec, const dampr_json_members *members);
+int32_t dampr_text_json_fields_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
+                                       uint64_t own_hi, const dampr_fields_spec *spec,
+                                       const dampr_json_members *members, dampr_kv *rec);
 /* compact the table into caller memory: codes[i], counts[i], reps[i] (rep = offset<<20 | len of the
  * lowest-offset occurrence, hashed tokens only, else 0). cap = array capacity; *n = entries written.
  * Pass all three arrays NULL to query *n only. Order is unspecified (dampr_table_to_kv +

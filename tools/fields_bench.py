@@ -26,10 +26,17 @@ MB/s, the stats line with filtered=N, and whether the host-map sample of the fil
 --sep ws writes the same rows with their fields joined by runs of 1-3 spaces or tabs instead of commas, a blank in
 front of about a quarter of them and behind another quarter (the filler field gives up the bytes, so every line keeps
 its LINE bytes), and runs the same pipelines with `l.split()`. The JSON line then also holds "sep": "ws".
+
+--format json writes JSON lines of JLINE bytes instead: {"user": "u%07d", "n": int, "status": an int or a string,
+"latency": float, "meta": {"user": "decoy", ...}, "pad": filler}, padded with JSON whitespace after the numbers, and
+runs `Dampr.json`-style stages: `map(json.loads).fold_by(r["user"], value=r["n"], +)` (--value float:
+float(r["latency"])), min / max / mean() the same way. The host-map rate is then json.loads plus the lambdas. The JSON
+line holds "format": "json"; --where is not taken.
 """
 import argparse
 import json
 import os
+import random
 import shutil
 import subprocess
 import sys
@@ -122,6 +129,33 @@ def whitespace_rows(text, seed, vwidth):
     return text
 
 
+JLINE = 176         # bytes per JSON line (--format json)
+
+
+def json_text(seed, n_lines, n_keys):
+    """n_lines seeded JSON lines of JLINE bytes: rows drawn from a pool of 4096 (int n, int-or-string status, float
+    latency, a nested decoy member named "user", a filler string), the user key u0000000..u{n_keys-1} (uniform)"""
+    prng = random.Random(seed)
+    pool = np.empty((4096, JLINE), dtype=np.uint8)
+    for i in range(len(pool)):
+        row = '{"user":"u0000000","n":%s,"status":%s,"latency":%s,"meta":{"user":"decoy","ids":[%d,%d]},"pad":"' % (
+            str(prng.randrange(-99999, 100000)).ljust(7), str(prng.choice([200, 201, 404, 500, '"404"', '"503"'])).ljust(6),
+            repr(prng.uniform(0, 1e3)).ljust(23), prng.randrange(1000), prng.randrange(1000))
+        row += "".join(prng.choice("abcdefghij") for _ in range(JLINE - 3 - len(row))) + '"}\n'
+        pool[i] = np.frombuffer(row.encode("ascii"), dtype=np.uint8)
+    at = row.index("u0000000") + 1
+    rng = np.random.default_rng(seed)
+    out = np.empty((n_lines, JLINE), dtype=np.uint8)
+    step = 1 << 20
+    for a in range(0, n_lines, step):
+        t = out[a:a + step]
+        t[:] = pool[rng.integers(0, len(pool), size=len(t))]
+        keys = rng.integers(0, n_keys, size=len(t))
+        for p in range(7):
+            t[:, at + 6 - p] = 48 + (keys // 10 ** p) % 10
+    return out.reshape(-1)
+
+
 SET_KEYS = tuple("u%07d" % (i * 7919) for i in range(64))
 WHERE = {"str": lambda r: r[0] < "u0500000", "int": lambda r: int(r[2]) >= 0, "float": lambda r: float(r[2]) >= 0,
          "set": lambda r: r[0] not in SET_KEYS}
@@ -131,7 +165,27 @@ def splitter(sep):
     return (lambda l: l.split()) if sep == "ws" else (lambda l: l.split(","))
 
 
+def json_job(Dampr, src, value, op):
+    d = Dampr.read_input(src).map(json.loads)
+    key = lambda r: r["user"]   # noqa: E731
+    val = (lambda r: r["n"]) if value == "int" else (lambda r: float(r["latency"]))
+    if op == "mean":
+        return d.mean(key, val)
+    if op in ("min", "max"):
+        return d.a_group_by(key, val).reduce(min if op == "min" else max)
+    return d.fold_by(key, value=val, binop=lambda a, b: a + b)
+
+
+def json_rows(sample, value):
+    """(key, value) of the sample's JSON lines, as the stage's lambdas read them"""
+    for l in sample.decode("ascii").split("\n")[:-1]:
+        r = json.loads(l)
+        yield r["user"], (r["n"] if value == "int" else float(r["latency"]))
+
+
 def job(Dampr, src, value="int", op="sum", where="none", sep="comma"):
+    if sep == "json":
+        return json_job(Dampr, src, value, op)
     conv = int if value == "int" else float
     d = Dampr.read_input(src).map(splitter(sep))
     if where != "none":
@@ -149,11 +203,11 @@ def python_fold(sample, value, op, where="none", sep="comma"):
     keep = WHERE.get(where, lambda r: True)
     split = splitter(sep)
     out = {}
-    for l in sample.decode("ascii").split("\n")[:-1]:
-        r = split(l)
-        if not keep(r):
-            continue
-        k, v = r[0], conv(r[2])
+    if sep == "json":
+        rows = json_rows(sample, value)
+    else:
+        rows = ((r[0], conv(r[2])) for r in map(split, sample.decode("ascii").split("\n")[:-1]) if keep(r))
+    for k, v in rows:
         if op == "mean":
             s, n = out.get(k, (0, 0))
             out[k] = (s + v, n + 1)
@@ -170,10 +224,11 @@ def magnitudes(sample, sep="comma"):
     """{key: (lines, sum of |float value|)} of the sample: the scale of the sum bound"""
     mag = {}
     split = splitter(sep)
-    for l in sample.decode("ascii").split("\n")[:-1]:
-        r = split(l)
-        n, a = mag.get(r[0], (0, 0.0))
-        mag[r[0]] = (n + 1, a + abs(float(r[2])))
+    rows = json_rows(sample, "float") if sep == "json" else \
+        ((r[0], r[2]) for r in map(split, sample.decode("ascii").split("\n")[:-1]))
+    for k, v in rows:
+        n, a = mag.get(k, (0, 0.0))
+        mag[k] = (n + 1, a + abs(float(v)))
     return mag
 
 
@@ -210,8 +265,15 @@ def main():
     ap.add_argument("--value", choices=("int", "float"), default="int")
     ap.add_argument("--op", choices=("sum", "min", "max", "mean"), default="sum")
     ap.add_argument("--where", choices=("none", "str", "int", "float", "set"), default="none")
-    ap.add_argument("--sep", choices=("comma", "ws"), default="comma")
+    ap.add_argument("--sep", choices=("comma", "ws", ","), default="comma")
+    ap.add_argument("--format", choices=("csv", "json"), default="csv")
     a = ap.parse_args()
+    if a.sep == ",":
+        a.sep = "comma"
+    if a.format == "json":
+        if a.where != "none" or a.sep != "comma":
+            ap.error("--format json takes neither --where nor --sep")
+        a.sep = "json"
     if a.where == "int" and a.value != "int":
         ap.error("--where int needs --value int (int() of a float field raises)")
     default = a.value == "int" and a.op == "sum"
@@ -220,8 +282,12 @@ def main():
     from dampr_b200 import runner as runner_mod
     ctx = runner_mod.get_ctx()
     name, power = card()
-    n_lines = int(a.gb * 1e9) // LINE
-    text = csv_text(2026, n_lines, a.keys) if a.value == "int" else float_text(2026, n_lines, a.keys)
+    line = JLINE if a.sep == "json" else LINE
+    n_lines = int(a.gb * 1e9) // line
+    if a.sep == "json":
+        text = json_text(2026, n_lines, a.keys)
+    else:
+        text = csv_text(2026, n_lines, a.keys) if a.value == "int" else float_text(2026, n_lines, a.keys)
     if a.sep == "ws":
         text = whitespace_rows(text, 2027, 6 if a.value == "int" else FVAL)
     nbytes = len(text)
@@ -261,10 +327,10 @@ def main():
     ctx.timing_enable(False)
 
     # host map on a sample: the stage as plain Python (the same lambdas), and the device result of the same bytes
-    sample_lines = max(1, int(a.sample_mb * 1e6) // LINE)
-    sample = pin.array[:sample_lines * LINE].tobytes()
+    sample_lines = max(1, int(a.sample_mb * 1e6) // line)
+    sample = pin.array[:sample_lines * line].tobytes()
     t0 = time.perf_counter()
-    if default:
+    if default and a.sep != "json":
         host = {}
         split = splitter(a.sep)
         for l in sample.decode("ascii").split("\n")[:-1]:
@@ -322,6 +388,8 @@ def main():
         })
     if a.sep == "ws":
         res["sep"] = "ws"
+    if a.sep == "json":
+        res["format"] = "json"
     if a.out is None:
         shutil.rmtree(tmpdir, ignore_errors=True)
     print(json.dumps(res))
