@@ -47,6 +47,13 @@
 // whitespace or lies before the line (the class of the last byte is carried across the 4-byte steps), and ends at
 // the next whitespace byte or the line end. Pass 1 counts the starts (the field count: 0 for a blank line, so every
 // index is missing), pass 2 walks the class changes: change 2i opens field i, change 2i + 1 closes it.
+//
+// TUP (tuple keys `(r[i], int(r[j]), ...)`, a compile-time parameter of the separator-byte and WS scans): up to 4
+// components take bound slots in the same walk as the predicates. The key code streams hash_bytes' two states over
+// the components (str bytes, the 8 bytes of v ^ 2^63 of an int, 0xFF between them). Components are not adjacent in
+// the line, so the representative is the line itself (offset << 20 | length, atomicMin keeps the lowest); an insert
+// that finds another line there splits that line again in global memory and compares the components (same_tuple).
+// table_tuple_keys_kernel decodes a tuple table the same way, from each entry's representative line.
 #include "common.cuh"
 #include "fparse.cuh"
 
@@ -437,11 +444,158 @@ __device__ __forceinline__ u64 hash_bytes(const u8 *p, u32 len, u64 seed) {
     return mix64((((u64)h1) << 32 | h2) ^ ((u64)len * 0x9E3779B97F4A7C15ULL)) | 0x8000000000000000ULL;
 }
 
+// ---- tuple keys ------------------------------------------------------------------------------------------------
+constexpr int T_MAX = DAMPR_FIELD_KEYS_MAX;
+
+// the components of a tuple-key scan, passed by value in the kernel parameters
+struct TupleView {
+    int field[T_MAX];
+    int is_int[T_MAX];
+    int n;
+};
+
+// the parameters of a tuple-key build: its predicates (n = 0 in a plain build) and components. fields_tiles takes the
+// address of `where` (a pointer to the first member of this standard-layout struct) and finds `tup` behind it.
+struct TupleWhere {
+    WhereView where;
+    TupleView tup;
+};
+
+// a tuple-key line's components: field ci[j] (-1: no component j, or it is missing: `missing`), bounds
+// [cs[j], ce[j]) in the window; nothing in the other builds
+template <bool TUP>
+struct TupleBounds {};
+template <>
+struct TupleBounds<true> {
+    int ci[T_MAX];
+    u32 cs[T_MAX], ce[T_MAX];
+    bool missing = false;
+};
+
+// hash_bytes' two running states after one more byte v
+__device__ __forceinline__ void hash_step(u32 &h1, u32 &h2, u32 v) {
+    h1 = (h1 ^ v) * 16777619u;
+    h2 = (h2 ^ v) * 0x85EBCA6Bu + 0x9E3779B9u;
+    h2 = (h2 << 13) | (h2 >> 19);
+}
+
+// the tuple's key code from its component bounds [cs[j], ce[j]) in t (see the header); false when an int()
+// component is not one the device parses (the host raises or decides)
+__device__ __forceinline__ bool tuple_code(const u8 *t, const u32 (&cs)[T_MAX], const u32 (&ce)[T_MAX],
+                                           const TupleView &tv, u64 seed, u64 &code) {
+    u32 h1 = (u32)seed ^ 0x811C9DC5u, h2 = (u32)(seed >> 32) ^ 0x9747B28Cu, len = 0;
+#pragma unroll
+    for (int j = 0; j < T_MAX; ++j) {
+        if (j < tv.n) {
+            if (j) {
+                hash_step(h1, h2, 0xFFu);
+                ++len;
+            }
+            if (tv.is_int[j]) {
+                long long v;
+                if (!parse_int(t + cs[j], ce[j] - cs[j], v)) return false;
+                const u64 x = (u64)v ^ 0x8000000000000000ULL;
+#pragma unroll
+                for (int b = 0; b < 8; ++b) hash_step(h1, h2, (u32)(x >> (8 * b)) & 0xFFu);
+                len += 8;
+            } else {
+                for (u32 i = cs[j]; i < ce[j]; ++i) hash_step(h1, h2, t[i]);
+                len += ce[j] - cs[j];
+            }
+        }
+    }
+    code = mix64((((u64)h1) << 32 | h2) ^ ((u64)len * 0x9E3779B97F4A7C15ULL)) | 0x8000000000000000ULL;
+    return true;
+}
+
+__device__ __forceinline__ bool is_split_ws(u32 c) { return (c - 0x09u) <= 4u || (c - 0x1Cu) <= 4u; }
+
+// bounds [s[j], e[j]) of the tuple's components in the taken line p[0, len) (every component exists), split by
+// the byte sep or (WS) by runs of str.split() whitespace, one byte at a time
+template <bool WS>
+__device__ __forceinline__ void line_fields(const u8 *p, u32 len, u32 sep, const TupleView &tv, u32 (&s)[T_MAX],
+                                            u32 (&e)[T_MAX]) {
+    int nf = WS ? 0 : 1;
+    bool prev_ws = true;
+    for (u32 i = 0; i < len; ++i) {
+        const u32 c = p[i];
+        if constexpr (WS) {
+            const bool w = is_split_ws(c);
+            nf += !w && prev_ws;
+            prev_ws = w;
+        } else {
+            nf += c == sep;
+        }
+    }
+    int want[T_MAX];
+#pragma unroll
+    for (int j = 0; j < T_MAX; ++j) {
+        want[j] = j < tv.n ? (tv.field[j] < 0 ? tv.field[j] + nf : tv.field[j]) : -1;
+        s[j] = e[j] = 0;
+    }
+    int f = WS ? -1 : 0;
+    u32 start = 0;
+    prev_ws = true;
+    for (u32 i = 0; i <= len; ++i) {
+        const u32 c = i < len ? p[i] : (WS ? 0x20u : sep);   // the line end closes the last field
+        bool close = false;
+        if constexpr (WS) {
+            const bool w = is_split_ws(c);
+            if (!w && prev_ws) {
+                ++f;
+                start = i;
+            }
+            close = w && !prev_ws;
+            prev_ws = w;
+        } else {
+            close = c == sep;
+        }
+        if (close) {
+#pragma unroll
+            for (int j = 0; j < T_MAX; ++j)
+                if (want[j] == f) {
+                    s[j] = start;
+                    e[j] = i;
+                }
+            if constexpr (!WS) {
+                ++f;
+                start = i + 1;
+            }
+        }
+    }
+}
+
+// the guard: the components of this line (bounds in t) against those of the representative line `other` (global
+// memory, taken by the device earlier, so its split cannot fail): str as bytes, int() as values
+template <bool WS>
+__device__ __forceinline__ bool same_tuple(const u8 *text, u64 other, const u8 *t, const u32 (&cs)[T_MAX],
+                                           const u32 (&ce)[T_MAX], const TupleView &tv, u32 sep) {
+    const u8 *o = text + (other >> 20);
+    u32 os[T_MAX], oe[T_MAX];
+    line_fields<WS>(o, (u32)(other & 0xFFFFFu), sep, tv, os, oe);
+    bool same = true;
+#pragma unroll
+    for (int j = 0; j < T_MAX; ++j) {
+        if (j < tv.n && same) {
+            const u32 la = ce[j] - cs[j], lb = oe[j] - os[j];
+            if (tv.is_int[j]) {
+                long long a = 0, b = 0;
+                same = parse_int(t + cs[j], la, a) && parse_int(o + os[j], lb, b) && a == b;
+            } else {
+                same = la == lb;
+                for (u32 i = 0; i < la && same; ++i) same = t[cs[j] + i] == o[os[j] + i];
+            }
+        }
+    }
+    return same;
+}
+
 // fold (code -> value) into the global table; false if a hashed key's representative is a different string.
-// F64: v holds the bits of a double (MIN / MAX only)
-template <bool F64>
+// F64: v holds the bits of a double (MIN / MAX only). LINE_REP (tuple keys): the representative is a line, and
+// when the entry's is another line than rep it goes to *other for the caller's guard (same_tuple)
+template <bool F64, bool LINE_REP = false>
 __device__ __forceinline__ bool fold_insert(const FieldsView &t, const u8 *text, u64 code, long long v, u64 rep,
-                                            u32 &flags) {
+                                            u32 &flags, u64 *other = nullptr) {
     u64 slot = mix64(code) & t.mask;
     for (u32 probe = 0; probe < F_G_MAX_PROBES; ++probe) {
         u64 k = *((volatile u64 *)&t.keys[slot]);
@@ -465,6 +619,10 @@ __device__ __forceinline__ bool fold_insert(const FieldsView &t, const u8 *text,
             if (rep == ~0ULL) return true;
             const u64 old = atomicMin(&t.reps[slot], rep);
             if (old == ~0ULL || old == rep) return true;
+            if constexpr (LINE_REP) {
+                *other = old;
+                return true;
+            }
             const u32 len = (u32)(rep & 0xFFFFFu);
             if ((u32)(old & 0xFFFFFu) != len) return false;
             const u8 *a = text + (rep >> 20), *b = text + (old >> 20);
@@ -608,8 +766,10 @@ __device__ __forceinline__ void json_fold(const u8 *t, u32 q, u32 end, u64 g0, c
 }
 
 // the kernel body over the tiles of [own_lo, own_hi); where: the predicates of a WHERE scan; WS: split on runs of
-// whitespace (`line.split()`) instead of the separator byte; JSON: json.loads each line and read the members *json
-template <int VK, int MODE, bool WHERE, bool WS, bool JSON = false>
+// whitespace (`line.split()`) instead of the separator byte; JSON: json.loads each line and read the members *json;
+// TUP: the key is the tuple of the components that follow the predicates (where points into a TupleWhere;
+// tab.key_field is component 0's field, tab.key_int is not read)
+template <int VK, int MODE, bool WHERE, bool WS, bool JSON = false, bool TUP = false>
 __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi,
                                              const FieldsView &tab, const RecView &rv, const WhereView *where,
                                              const JsonView *json = nullptr) {
@@ -741,6 +901,8 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
             bool dropped = false;   // WHERE: a predicate is false
             long long val = 1, kval = 0;
             u64 code = 0, rep = ~0ULL;
+            TupleBounds<TUP> kb;   // TUP: the key components' fields and bounds
+            const TupleView *tup = TUP ? &reinterpret_cast<const TupleWhere *>(where)->tup : nullptr;
             if constexpr (JSON) {
                 if (!to_host) json_fold<VK, WHERE>(s.text, q, end, gq - q, tab, *json, where, to_host, dropped, val, code,
                                                    rep, acc_long, my_flags);
@@ -751,6 +913,22 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                 const bool one = tab.val_field == DAMPR_FIELD_VAL_ONE;
                 const int vi = one ? 0 : (tab.val_field < 0 ? tab.val_field + nf : tab.val_field);
                 const bool kv_missing = ki < 0 || ki >= nf || vi < 0 || vi >= nf;
+                if constexpr (TUP) {   // (tab.key_field is component 0's field: kv_missing covers it)
+#pragma unroll
+                    for (int j = 0; j < T_MAX; ++j) {
+                        int i = -1;
+                        if (j < tup->n) {
+                            i = tup->field[j] < 0 ? tup->field[j] + nf : tup->field[j];
+                            if (i < 0 || i >= nf) {
+                                kb.missing = true;
+                                i = -1;
+                            }
+                        }
+                        kb.ci[j] = i;
+                        kb.cs[j] = !WS && i == 0 ? q : 0xFFFFFFFFu;
+                        kb.ce[j] = i >= 0 && i == nf - 1 ? end : 0xFFFFFFFFu;
+                    }
+                }
                 if (!WHERE && kv_missing) {
                     to_host = true;   // IndexError: Python raises it
                 } else {
@@ -776,6 +954,10 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                             pe[j] = pi[j] == nf - 1 ? end : 0xFFFFFFFFu;
                             need = max(need, pi[j] + 1);
                         }
+                    }
+                    if constexpr (TUP) {
+#pragma unroll
+                        for (int j = 0; j < T_MAX; ++j) need = max(need, kb.ci[j] + 1);
                     }
                     int f = 0;
                     skip = q & 3u;
@@ -806,6 +988,11 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                                         for (int j = 0; j < P_MAX; ++j)
                                             if (fi == pi[j]) pe[j] = p;
                                     }
+                                    if constexpr (TUP) {
+#pragma unroll
+                                        for (int j = 0; j < T_MAX; ++j)
+                                            if (fi == kb.ci[j]) kb.ce[j] = p;
+                                    }
                                 } else {
                                     if (fi == ki) ks = p;
                                     if (fi == vi) vs = p;
@@ -813,6 +1000,11 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
 #pragma unroll
                                         for (int j = 0; j < P_MAX; ++j)
                                             if (fi == pi[j]) ps[j] = p;
+                                    }
+                                    if constexpr (TUP) {
+#pragma unroll
+                                        for (int j = 0; j < T_MAX; ++j)
+                                            if (fi == kb.ci[j]) kb.cs[j] = p;
                                     }
                                 }
                                 ++f;
@@ -838,6 +1030,11 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                                     for (int j = 0; j < P_MAX; ++j)
                                         if (f == pi[j]) pe[j] = p;
                                 }
+                                if constexpr (TUP) {
+#pragma unroll
+                                    for (int j = 0; j < T_MAX; ++j)
+                                        if (f == kb.ci[j]) kb.ce[j] = p;
+                                }
                                 ++f;
                                 if (f == ki) ks = p + 1;
                                 if (f == vi) vs = p + 1;
@@ -845,6 +1042,11 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
 #pragma unroll
                                     for (int j = 0; j < P_MAX; ++j)
                                         if (f == pi[j]) ps[j] = p + 1;
+                                }
+                                if constexpr (TUP) {
+#pragma unroll
+                                    for (int j = 0; j < T_MAX; ++j)
+                                        if (f == kb.ci[j]) kb.cs[j] = p + 1;
                                 }
                             }
                         }
@@ -871,7 +1073,13 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                             to_host = true;
                         }
                         if (!to_host) {
-                            if (tab.key_int) {
+                            if constexpr (TUP) {
+                                // a missing component other than the first is an IndexError: Python raises it
+                                if (!kb.missing && tuple_code(s.text, kb.cs, kb.ce, *tup, tab.seed, code))
+                                    rep = (gq << 20) | (end - q);
+                                else
+                                    to_host = true;
+                            } else if (tab.key_int) {
                                 if (!parse_int(s.text + ks, klen, kval)) to_host = true;
                                 else code = (u64)kval ^ 0x8000000000000000ULL;
                             } else if (klen >= 1 && klen <= 9) {
@@ -921,7 +1129,17 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                 my_flags |= DAMPR_TF_NEGZERO;
             }
             bool same;
-            if constexpr (MODE == M_RECORDS) {
+            if constexpr (TUP) {
+                // the guard re-splits the entry's representative line when it is another one than this line
+                u64 other = ~0ULL;
+                if constexpr (MODE == M_RECORDS) {
+                    put_record(rv, tbase + li, code, (u64)val, my_flags);
+                    same = fold_insert<false, true>(tab, text, code, 1, rep, my_flags, &other);
+                } else {
+                    same = fold_insert<VK == VK_F64, true>(tab, text, code, val, rep, my_flags, &other);
+                }
+                if (other != ~0ULL) same = same_tuple<WS>(text, other, s.text, kb.cs, kb.ce, *tup, tab.sep);
+            } else if constexpr (MODE == M_RECORDS) {
                 put_record(rv, tbase + li, code, (u64)val, my_flags);
                 same = fold_insert<false>(tab, text, code, 1, rep, my_flags);   // the line count of the key
             } else {
@@ -992,16 +1210,38 @@ text_json_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_
 }
 static_assert(sizeof(WhereView) + sizeof(JsonView) + 256 <= 4096, "kernel parameters");
 
+// the tuple-key builds (plain and WHERE) of the separator-byte and whitespace scans: the components (and the
+// predicates, unused by a plain build) read in place from the parameters. As for the JSON builds, saying that the
+// plain builds run 4 CTAs per SM keeps ptxas from squeezing them into 40 registers and spilling.
+template <int VK, int MODE, bool WHERE, bool WS>
+__global__ void __launch_bounds__(F_THREADS, WHERE ? 1 : 4)
+text_fields_tuple_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv,
+                         const __grid_constant__ TupleWhere tw) {
+    static_assert(MODE != M_COUNT, "the count pass is the plain kernel's");
+    fields_tiles<VK, MODE, WHERE, WS, false, true>(text, n, own_lo, own_hi, tab, rv, &tw.where);
+}
+static_assert(sizeof(TupleWhere) + 256 <= 4096, "kernel parameters");
+
 // one kernel over the tiles of [own_lo, own_hi); WHERE: the build that applies the predicates *wh; WS: the
-// whitespace-split build; JSON: the JSON-lines build over the members *jv
-template <int VK, int MODE, bool WHERE = false, bool WS = false, bool JSON = false>
+// whitespace-split build; JSON: the JSON-lines build over the members *jv; TUP: the tuple-key build over *tk
+template <int VK, int MODE, bool WHERE = false, bool WS = false, bool JSON = false, bool TUP = false>
 int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const FieldsView &tv, const RecView &rv,
-                  int timer, const WhereView *wh = nullptr, const JsonView *jv = nullptr) {
+                  int timer, const WhereView *wh = nullptr, const JsonView *jv = nullptr,
+                  const TupleView *tk = nullptr) {
     const size_t smem = sizeof(SmemF);
     const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
     u64 grid = (u64)ctx->num_sms * 4;
     if (grid > ntiles) grid = ntiles;
-    if constexpr (JSON && WHERE) {
+    if constexpr (TUP) {
+        TupleWhere tw{};
+        if (wh) tw.where = *wh;
+        tw.tup = *tk;
+        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, TupleWhere) =
+            text_fields_tuple_kernel<VK, MODE, WHERE, WS>;
+        CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ScopedTimer tm(ctx, timer);
+        kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, tw);
+    } else if constexpr (JSON && WHERE) {
         void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonView, WhereView) =
             text_json_fields_kernel<VK, MODE>;
         CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1129,15 +1369,20 @@ FieldsView fields_view(dampr_table *t, const dampr_fields_spec *spec, int op) {
 }
 
 // the fold pass of one range under one separator class: the plain kernel, or its WHERE build when spec holds
-// predicates
+// predicates; tk: the tuple-key builds over those components
 template <int VK, int MODE, bool WS>
 int launch_fold_sep(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
-                    const FieldsView &tv, const RecView &rv) {
-    if (spec->npreds == 0)
-        return launch_fields<VK, MODE, false, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS);
+                    const FieldsView &tv, const RecView &rv, const TupleView *tk) {
+    if (spec->npreds == 0) {
+        if (!tk) return launch_fields<VK, MODE, false, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS);
+        return launch_fields<VK, MODE, false, WS, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS,
+                                                               nullptr, nullptr, tk);
+    }
     WhereView w;
     if (int r = where_view(ctx, spec, w)) return r;
-    return launch_fields<VK, MODE, true, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w);
+    if (!tk) return launch_fields<VK, MODE, true, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w);
+    return launch_fields<VK, MODE, true, WS, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w,
+                                                          nullptr, tk);
 }
 
 // the fold pass of one range of a JSON scan: the plain build reads two members, the WHERE build (also taken without
@@ -1156,9 +1401,90 @@ int launch_json_fold(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, 
 // the fold pass of one range: the separator-byte build, or the whitespace-split one under DAMPR_FIELD_SEP_WS
 template <int VK, int MODE>
 int launch_fold(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
-                const FieldsView &tv, const RecView &rv) {
-    if (spec->sep == DAMPR_FIELD_SEP_WS) return launch_fold_sep<VK, MODE, true>(ctx, tb, own_lo, own_hi, spec, tv, rv);
-    return launch_fold_sep<VK, MODE, false>(ctx, tb, own_lo, own_hi, spec, tv, rv);
+                const FieldsView &tv, const RecView &rv, const TupleView *tk = nullptr) {
+    if (spec->sep == DAMPR_FIELD_SEP_WS)
+        return launch_fold_sep<VK, MODE, true>(ctx, tb, own_lo, own_hi, spec, tv, rv, tk);
+    return launch_fold_sep<VK, MODE, false>(ctx, tb, own_lo, own_hi, spec, tv, rv, tk);
+}
+
+// the components of a tuple-key call in kernel-parameter form
+int tuple_view(dampr_ctx *ctx, const dampr_field_keys *keys, TupleView &tk) {
+    ARG_CHECK(ctx, keys != nullptr, "null");
+    ARG_CHECK(ctx, keys->n >= 1 && keys->n <= T_MAX, "1 .. DAMPR_FIELD_KEYS_MAX key components");
+    tk = TupleView{};
+    tk.n = keys->n;
+    for (int j = 0; j < keys->n; ++j) {
+        ARG_CHECK(ctx, keys->kind[j] == DAMPR_FIELD_KEY_STR || keys->kind[j] == DAMPR_FIELD_KEY_INT,
+                  "key component kind");
+        tk.field[j] = keys->field[j];
+        tk.is_int[j] = keys->kind[j] == DAMPR_FIELD_KEY_INT;
+    }
+    return DAMPR_OK;
+}
+
+// fields_view of a tuple-key call: its key field is component 0's (the scan's missing-field rule checks it with the
+// value field; the tuple build checks the others)
+FieldsView tuple_fields_view(dampr_table *t, const dampr_fields_spec *spec, int op, const TupleView &tk) {
+    FieldsView tv = fields_view(t, spec, op);
+    tv.key_field = tk.field[0];
+    tv.key_int = 0;
+    return tv;
+}
+
+// the columns of dampr_table_fetch_field_keys on the device
+struct TupleCols {
+    u8 *str[T_MAX];
+    long long *ints[T_MAX];
+    u32 width[T_MAX];
+};
+
+// one entry of a tuple-key table per thread: its representative line split again. maxlen != nullptr: the longest
+// str component of each column only; else the entry's row (compacted through cursor) of every column
+template <bool WS>
+__global__ void table_tuple_keys_kernel(const u64 *__restrict__ keys, const u64 *__restrict__ counts,
+                                        const u64 *__restrict__ reps, u64 cap, const u8 *__restrict__ text, u32 sep,
+                                        const __grid_constant__ TupleView tv, const __grid_constant__ TupleCols out,
+                                        u64 *out_counts, u64 *out_codes, u64 out_cap, u64 *cursor, u32 *maxlen) {
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = blockIdx.x * (u64)blockDim.x + threadIdx.x; i < cap; i += stride) {
+        const u64 k = keys[i];
+        const bool have = k != 0;
+        u64 idx = 0;
+        if (!maxlen) {
+            const u32 m = __ballot_sync(0xFFFFFFFFu, have);
+            u64 base = 0;
+            if (m) {
+                const int leader = __ffs(m) - 1;
+                if ((int)(threadIdx.x & 31) == leader) base = atomicAdd(cursor, (u64)__popc(m));
+                base = __shfl_sync(0xFFFFFFFFu, base, leader);
+            }
+            idx = base + __popc(m & ((1u << (threadIdx.x & 31)) - 1u));
+        }
+        if (!have || (!maxlen && idx >= out_cap)) continue;
+        const u64 rep = reps[i];
+        const u8 *p = text + (rep >> 20);
+        u32 s[T_MAX], e[T_MAX];
+        line_fields<WS>(p, (u32)(rep & 0xFFFFFu), sep, tv, s, e);
+#pragma unroll
+        for (int j = 0; j < T_MAX; ++j) {
+            if (j >= tv.n) continue;
+            if (maxlen) {
+                if (!tv.is_int[j]) atomicMax(&maxlen[j], e[j] - s[j]);
+            } else if (tv.is_int[j]) {
+                long long v = 0;
+                parse_int(p + s[j], e[j] - s[j], v);
+                out.ints[j][idx] = v;
+            } else {
+                const u32 w = out.width[j], len = min(e[j] - s[j], w);
+                u8 *o = out.str[j] + idx * w;
+                for (u32 b = 0; b < len; ++b) o[b] = p[s[j] + b];
+                for (u32 b = len; b < w; ++b) o[b] = 0;
+            }
+        }
+        if (maxlen) continue;
+        if (out_counts) out_counts[idx] = counts[i];
+        if (out_codes) out_codes[idx] = k;
+    }
 }
 
 // record mode's first two kernels over one range: lines per tile (the tile array grown to the range), then the
@@ -1250,4 +1576,134 @@ extern "C" int32_t dampr_text_json_fields_records(dampr_ctx *ctx, dampr_table *t
     if (spec->op == DAMPR_OP_SUM_F64)
         return launch_json_fold<VK_F64, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, jv, tv, rv);
     return launch_json_fold<VK_INT, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, jv, tv, rv);
+}
+
+extern "C" int32_t dampr_text_fields_tuple(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
+                                           uint64_t own_hi, const dampr_fields_spec *spec,
+                                           const dampr_field_keys *keys) {
+    if (int r = check_fields_args(ctx, t, tb, own_lo, own_hi, spec)) return r;
+    TupleView tk;
+    if (int r = tuple_view(ctx, keys, tk)) return r;
+    const bool f64 = spec->op == DAMPR_OP_MIN_F64 || spec->op == DAMPR_OP_MAX_F64;
+    ARG_CHECK(ctx, f64 || spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_MIN_I64 ||
+                       spec->op == DAMPR_OP_MAX_I64,
+              "op must be DAMPR_OP_SUM_I64, DAMPR_OP_MIN_I64, DAMPR_OP_MAX_I64, DAMPR_OP_MIN_F64 or DAMPR_OP_MAX_F64");
+    ARG_CHECK(ctx, !f64 || spec->val_field != DAMPR_FIELD_VAL_ONE, "a float op needs a value field");
+    if (own_hi <= own_lo) return DAMPR_OK;
+    const FieldsView tv = tuple_fields_view(t, spec, spec->op, tk);
+    wait_uploads(ctx);
+    if (f64) return launch_fold<VK_F64, M_TABLE>(ctx, tb, own_lo, own_hi, spec, tv, RecView{}, &tk);
+    return launch_fold<VK_INT, M_TABLE>(ctx, tb, own_lo, own_hi, spec, tv, RecView{}, &tk);
+}
+
+extern "C" int32_t dampr_text_fields_tuple_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb,
+                                                   uint64_t own_lo, uint64_t own_hi, const dampr_fields_spec *spec,
+                                                   const dampr_field_keys *keys, dampr_kv *rec) {
+    if (int r = check_fields_args(ctx, t, tb, own_lo, own_hi, spec)) return r;
+    TupleView tk;
+    if (int r = tuple_view(ctx, keys, tk)) return r;
+    ARG_CHECK(ctx, rec != nullptr, "null");
+    ARG_CHECK(ctx, spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_SUM_F64,
+              "op must be DAMPR_OP_SUM_I64 or DAMPR_OP_SUM_F64");
+    ARG_CHECK(ctx, spec->val_field != DAMPR_FIELD_VAL_ONE, "record mode needs a value field");
+    if (own_hi <= own_lo) return DAMPR_OK;
+    const FieldsView tv = tuple_fields_view(t, spec, DAMPR_OP_SUM_I64, tk);
+    RecView rv{rec->rec, rec->capacity, nullptr};
+    if (int r = count_records(ctx, t, tb, own_lo, own_hi, tv, rv)) return r;
+    if (spec->op == DAMPR_OP_SUM_F64) return launch_fold<VK_F64, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, tv, rv, &tk);
+    return launch_fold<VK_INT, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, tv, rv, &tk);
+}
+
+extern "C" int32_t dampr_table_fetch_field_keys(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, int32_t sep,
+                                                const dampr_field_keys *keys, uint32_t widths[DAMPR_FIELD_KEYS_MAX],
+                                                void *const cols[DAMPR_FIELD_KEYS_MAX], uint64_t *counts,
+                                                uint64_t *codes, uint64_t cap, uint64_t *n) {
+    ARG_CHECK(ctx, ctx && t && tb && n && widths, "null");
+    ARG_CHECK(ctx, sep == DAMPR_FIELD_SEP_WS || (sep > 0 && sep < 0x80 && sep != '\n' && sep != '\r'),
+              "separator must be DAMPR_FIELD_SEP_WS or an ASCII byte other than NUL, '\\n' and '\\r'");
+    TupleView tk;
+    if (int r = tuple_view(ctx, keys, tk)) return r;
+    uint64_t st[8];
+    if (int r = dampr_table_stats(ctx, t, st)) return r;
+    const u64 m = *n = st[0];
+    const bool ws = sep == DAMPR_FIELD_SEP_WS;
+    const unsigned grid = ctx->num_sms * 4;
+    if (!cols) {   // phase 1: the longest str component of each column
+        for (int j = 0; j < T_MAX; ++j) widths[j] = 0;
+        if (m == 0) return DAMPR_OK;
+        u32 *d = (u32 *)pool_alloc(ctx, T_MAX * sizeof(u32));
+        ARG_CHECK(ctx, d != nullptr, "device allocation failed");
+        cudaError_t e = cudaMemsetAsync(d, 0, T_MAX * sizeof(u32), ctx->stream);
+        if (e == cudaSuccess) {
+            ScopedTimer tm(ctx, DAMPR_K_TABLE_EXTRACT);
+            if (ws)
+                table_tuple_keys_kernel<true><<<grid, 256, 0, ctx->stream>>>(
+                    t->keys, t->counts, t->reps, t->cap, tb->text, (u32)sep, tk, TupleCols{}, nullptr, nullptr, 0,
+                    nullptr, d);
+            else
+                table_tuple_keys_kernel<false><<<grid, 256, 0, ctx->stream>>>(
+                    t->keys, t->counts, t->reps, t->cap, tb->text, (u32)sep, tk, TupleCols{}, nullptr, nullptr, 0,
+                    nullptr, d);
+            e = cudaGetLastError();
+        }
+        u32 w[T_MAX];
+        if (e == cudaSuccess) e = cudaMemcpyAsync(w, d, sizeof w, cudaMemcpyDeviceToHost, ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+        pool_free(ctx, d);
+        if (e != cudaSuccess) {
+            ctx->err = std::string("table fetch_field_keys failed: ") + cudaGetErrorString(e);
+            return DAMPR_ERR_CUDA;
+        }
+        for (int j = 0; j < T_MAX; ++j) widths[j] = j < tk.n && !tk.is_int[j] ? w[j] : 0;
+        return DAMPR_OK;
+    }
+    ARG_CHECK(ctx, cap >= m, "fetch arrays too small");
+    if (m == 0) return DAMPR_OK;
+    // one pool block: the columns, then counts, codes and the cursor
+    u64 bytes[T_MAX], total = 0;
+    for (int j = 0; j < tk.n; ++j) {
+        ARG_CHECK(ctx, cols[j] != nullptr, "null column");
+        ARG_CHECK(ctx, tk.is_int[j] || (widths[j] >= 1 && widths[j] <= 0xFFFFFu), "a str column's width");
+        bytes[j] = tk.is_int[j] ? m * 8 : ((m * widths[j] + 7) & ~7ULL);
+        total += bytes[j];
+    }
+    u8 *d = (u8 *)pool_alloc(ctx, total + 2 * m * 8 + 8);
+    ARG_CHECK(ctx, d != nullptr, "device allocation failed");
+    TupleCols out{};
+    u64 off = 0;
+    for (int j = 0; j < tk.n; ++j) {
+        if (tk.is_int[j]) out.ints[j] = (long long *)(d + off);
+        else out.str[j] = d + off;
+        out.width[j] = tk.is_int[j] ? 0 : widths[j];
+        off += bytes[j];
+    }
+    u64 *d_counts = (u64 *)(d + total), *d_codes = d_counts + m, *d_cur = d_codes + m;
+    cudaError_t e = cudaMemsetAsync(d_cur, 0, 8, ctx->stream);
+    if (e == cudaSuccess) {
+        ScopedTimer tm(ctx, DAMPR_K_TABLE_EXTRACT);
+        if (ws)
+            table_tuple_keys_kernel<true><<<grid, 256, 0, ctx->stream>>>(
+                t->keys, t->counts, t->reps, t->cap, tb->text, (u32)sep, tk, out, d_counts, d_codes, m, d_cur,
+                nullptr);
+        else
+            table_tuple_keys_kernel<false><<<grid, 256, 0, ctx->stream>>>(
+                t->keys, t->counts, t->reps, t->cap, tb->text, (u32)sep, tk, out, d_counts, d_codes, m, d_cur,
+                nullptr);
+        e = cudaGetLastError();
+    }
+    off = 0;
+    for (int j = 0; j < tk.n && e == cudaSuccess; ++j) {
+        e = cudaMemcpyAsync(cols[j], d + off, tk.is_int[j] ? m * 8 : m * widths[j], cudaMemcpyDeviceToHost,
+                            ctx->stream);
+        off += bytes[j];
+    }
+    if (e == cudaSuccess && counts) e = cudaMemcpyAsync(counts, d_counts, m * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess && codes) e = cudaMemcpyAsync(codes, d_codes, m * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    pool_free(ctx, d);
+    if (e != cudaSuccess) {
+        ctx->err = std::string("table fetch_field_keys failed: ") + cudaGetErrorString(e);
+        return DAMPR_ERR_CUDA;
+    }
+    return DAMPR_OK;
 }

@@ -36,6 +36,7 @@ FIELD_SEP_WS = 256   # sep: split like str.split() (runs of ASCII whitespace, no
 FIELD_SEP_JSON = 257   # sep of the JSON-lines calls: fields are the members of json.loads(line)
 JSON_MAX_MEMBERS, JSON_MAX_NAME, JSON_MAX_DEPTH = 8, 64, 64
 FIELDS_HALO = 65536
+FIELD_KEYS_MAX = 4   # components of a tuple key (dampr_field_keys)
 # WHERE predicates of a field scan (dampr_field_pred): kinds, comparisons, limits per call
 PRED_STR, PRED_INT, PRED_F64, PRED_NFIELDS, PRED_MEMBER = range(5)
 CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_IN, CMP_NOT_IN = range(8)
@@ -100,6 +101,20 @@ def fields_spec(spec, cr_is_data, preds):
                    C.cast(arr, C.POINTER(FieldPred)), len(preds))
     s._keep = keep
     return s
+
+
+class FieldKeys(C.Structure):
+    """dampr_field_keys"""
+    _fields_ = [("n", C.c_int32), ("field", C.c_int32 * FIELD_KEYS_MAX), ("kind", C.c_int32 * FIELD_KEYS_MAX)]
+
+
+def field_keys(keys):
+    """dampr_field_keys of the tuple key components keys = [(field index, FIELD_KEY_STR | FIELD_KEY_INT)]"""
+    k = FieldKeys()
+    k.n = len(keys)
+    for j, (i, kind) in enumerate(keys[:FIELD_KEYS_MAX]):
+        k.field[j], k.kind[j] = int(i), int(kind)
+    return k
 
 
 class JsonMembers(C.Structure):
@@ -179,6 +194,10 @@ def load_library():
     _sig(lib, "dampr_text_json_fields", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), C.POINTER(JsonMembers))
     _sig(lib, "dampr_text_json_fields_records", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), C.POINTER(JsonMembers),
          vp)
+    _sig(lib, "dampr_text_fields_tuple", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), C.POINTER(FieldKeys))
+    _sig(lib, "dampr_text_fields_tuple_records", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), C.POINTER(FieldKeys), vp)
+    _sig(lib, "dampr_table_fetch_field_keys", vp, vp, vp, i32, C.POINTER(FieldKeys), C.POINTER(u32), C.POINTER(vp),
+         vp, vp, u64, pu64)
     _sig(lib, "dampr_table_stats", vp, vp, pu64)
     _sig(lib, "dampr_table_fallback_lines", vp, vp, vp, u64, pu64)
     _sig(lib, "dampr_table_fetch", vp, vp, vp, vp, vp, u64, pu64)
@@ -628,6 +647,41 @@ class Table(object):
         s, m = fields_spec(spec, cr_is_data, preds), json_members(members)
         self.ctx.check(self.ctx.lib.dampr_text_json_fields_records(self.ctx.h, self.h, tb.h, int(lo), int(hi),
                                                                    C.byref(s), C.byref(m), kv.h))
+
+    def fields_tuple(self, tb, lo, hi, spec, keys, cr_is_data=False, preds=()):
+        """fields() grouped by a tuple key: keys = [(field index, FIELD_KEY_STR | FIELD_KEY_INT)], 1 .. FIELD_KEYS_MAX
+        components on spec's separator (spec's key field and kind are not read)"""
+        s, k = fields_spec(spec, cr_is_data, preds), field_keys(keys)
+        self.ctx.check(self.ctx.lib.dampr_text_fields_tuple(self.ctx.h, self.h, tb.h, int(lo), int(hi), C.byref(s),
+                                                            C.byref(k)))
+
+    def fields_tuple_records(self, tb, lo, hi, spec, keys, kv, cr_is_data=False, preds=()):
+        """fields_records() grouped by a tuple key, keys as fields_tuple()"""
+        s, k = fields_spec(spec, cr_is_data, preds), field_keys(keys)
+        self.ctx.check(self.ctx.lib.dampr_text_fields_tuple_records(self.ctx.h, self.h, tb.h, int(lo), int(hi),
+                                                                    C.byref(s), C.byref(k), kv.h))
+
+    def fetch_field_keys(self, tb, sep, keys):
+        """(columns, counts, codes) of a tuple-key table, decoded on the device from each entry's representative line:
+        one column per component of keys (as fields_tuple()), an 'S<width>' array for str components and an int64
+        array for int() ones, all in one row order with the accumulators and key codes (uint64)"""
+        k = field_keys(keys)
+        widths, n = (C.c_uint32 * FIELD_KEYS_MAX)(), C.c_uint64(0)
+        self.ctx.check(self.ctx.lib.dampr_table_fetch_field_keys(self.ctx.h, self.h, tb.h, int(sep), C.byref(k), widths,
+                                                                 None, None, None, 0, C.byref(n)))
+        m = n.value
+        cols = [np.empty(m, dtype=np.int64) if kind == FIELD_KEY_INT else np.empty((m, max(1, widths[j])), np.uint8)
+                for j, (_i, kind) in enumerate(keys)]
+        counts, codes = np.empty(m, dtype=np.uint64), np.empty(m, dtype=np.uint64)
+        if m:
+            ptrs = (C.c_void_p * FIELD_KEYS_MAX)(*[_ptr(c) for c in cols])
+            for j, c in enumerate(cols):
+                widths[j] = c.shape[1] if c.ndim == 2 else 0
+            self.ctx.check(self.ctx.lib.dampr_table_fetch_field_keys(self.ctx.h, self.h, tb.h, int(sep), C.byref(k),
+                                                                     widths, ptrs, _ptr(counts), _ptr(codes), m,
+                                                                     C.byref(n)))
+        cols = [c.view("S%d" % c.shape[1]).ravel() if c.ndim == 2 else c for c in cols]
+        return cols, counts, codes
 
     def fields_stats(self):
         """stats() of a field scan under the names of its counters. "records" is the record count in record mode;

@@ -290,7 +290,11 @@ def _is_one(e):
     return ok and type(v) is int and v == 1
 
 
-def text_fields_spec(key_fn, value_fn, split_fn=None, whitespace=False):
+FIELD_TUPLE = "tuple"   # a key that is a tuple of field projections
+TUPLE_MAX = 4           # components of a tuple key the device takes (DAMPR_FIELD_KEYS_MAX)
+
+
+def text_fields_spec(key_fn, value_fn, split_fn=None, whitespace=False, tuple_keys=False):
     """Device field-scan spec of a keyed(key_fn, value_fn) over text lines, optionally behind map(split_fn):
     (sep, key_index, key_kind, value_index, value_kind, mean) where the key is l.split(sep)[key_index] (FIELD_STR) or
     its int() (FIELD_INT), and the value is
@@ -298,7 +302,10 @@ def text_fields_spec(key_fn, value_fn, split_fn=None, whitespace=False):
       int() or float() of l.split(sep)[value_index]    FIELD_INT or FIELD_FLOAT, mean False
       mean()'s `(value(v), 1)`, value one of those     FIELD_INT or FIELD_FLOAT, mean True
     Indices may be negative (Python's from-the-end). With `whitespace` the split may also be l.split() / l.split(None),
-    sep SEP_WS (a caller that only handles separator characters leaves it off). None for any other shape."""
+    sep SEP_WS (a caller that only handles separator characters leaves it off). With `tuple_keys` the key may also be
+    a tuple of 1 .. TUPLE_MAX such projections on the same split, e.g. (l.split(S)[0], int(l.split(S)[3])): key_kind
+    is then FIELD_TUPLE and key_index the components ((index, FIELD_STR | FIELD_INT), ...). None for any other
+    shape."""
     fns = [f for f in (key_fn, value_fn, split_fn) if f is not None]
     if not all(isinstance(f, types.FunctionType) and f.__code__.co_argcount == 1 for f in fns):
         return None
@@ -316,6 +323,11 @@ def text_fields_spec(key_fn, value_fn, split_fn=None, whitespace=False):
         def record(x):                           # key / value functions index the split record
             return sep if _is_arg(x) else None
     k = _field_proj(ke, record)
+    if k is None and tuple_keys and ke.op == "tuple" and 1 <= len(ke.a) <= TUPLE_MAX:
+        comps = [_field_proj(c, record) for c in ke.a]
+        if any(c is None for c in comps) or len({c[2] for c in comps}) != 1:
+            return None
+        k = FIELD_TUPLE, tuple((i, kind) for kind, i, _sep in comps), comps[0][2]
     if k is None:
         return None
     if _is_one(ve):

@@ -751,6 +751,8 @@ class FieldScan(TextScan):
     def __init__(self, runner, sources, spec, op, stage, mean, preds=()):
         TextScan.__init__(self, runner, sources, None)
         self.spec = spec     # (separator byte or FIELD_SEP_WS, key index, key kind, value index or FIELD_VAL_ONE)
+        # a tuple key (key kind KEY_TUPLE): its components go to the tuple calls, the spec's key field is not read
+        self.key_comps = spec[1] if spec[2] == KEY_TUPLE else None
         self.preds = preds   # the stage's filters as device WHERE predicates (device.fields_spec)
         self._where = {"preds": preds} if preds else {}
         self.filtered = 0    # lines the predicates dropped on the device
@@ -767,15 +769,24 @@ class FieldScan(TextScan):
 
     def _launch(self, tab, tb, lo, hi):
         spec = tuple(self.spec) + (self.op,)
+        cr = getattr(self, "_cr_is_data", False)
+        if self.key_comps is not None:
+            spec = (spec[0], 0, dev.FIELD_KEY_STR) + spec[3:]
         if not self.records:
             # a stage without filters makes exactly the plain call
-            tab.fields(tb, lo, hi, spec, getattr(self, "_cr_is_data", False), **self._where)
+            if self.key_comps is not None:
+                tab.fields_tuple(tb, lo, hi, spec, self.key_comps, cr, **self._where)
+            else:
+                tab.fields(tb, lo, hi, spec, cr, **self._where)
             return
         if self._rec is None:
             # a first guess of one record per 32 bytes of text; a scan with more lines is repeated once with a
             # buffer of the exact size (DAMPR_TF_RECFULL)
             self._records_buffer(min(tb.n // 32 + 4096, self._free_bytes() // (2 * self.REC_BYTES)))
-        tab.fields_records(tb, lo, hi, spec, self._rec, getattr(self, "_cr_is_data", False), **self._where)
+        if self.key_comps is not None:
+            tab.fields_tuple_records(tb, lo, hi, spec, self.key_comps, self._rec, cr, **self._where)
+        else:
+            tab.fields_records(tb, lo, hi, spec, self._rec, cr, **self._where)
 
     def _free_bytes(self):
         return int(self.runner.ctx.mem_info()[0])
@@ -823,7 +834,9 @@ class FieldScan(TextScan):
             self._rec_regrown = True
             self._records_buffer(int(st["records"]))   # the exact line count of the scan
             return self._run()
-        if self.spec[2] == dev.FIELD_KEY_INT:
+        if self.key_comps is not None:
+            keys, acc, codes = self._fetch_tuple_keys(tab, tb)
+        elif self.spec[2] == dev.FIELD_KEY_INT:
             codes, acc, _reps = tab.fetch()
             keys = (codes ^ np.uint64(1 << 63)).view(np.int64)
         elif self.records:
@@ -863,6 +876,13 @@ class FieldScan(TextScan):
         if self.preds:   # the table-mode slot, or the records that are neither folded nor handed back
             self.filtered = int(st["records"]) - (int(st["lines"]) + int(st["fallback"]) if self.records else 0)
         return self
+
+    def _fetch_tuple_keys(self, tab, tb):
+        """(list of key tuples, accumulators, key codes) of a tuple-key table: one column per component decoded on the
+        device, the tuples built in one zip"""
+        cols, acc, codes = tab.fetch_field_keys(tb, self.spec[0], self.key_comps)
+        cols = [c.astype("U%d" % c.dtype.itemsize).tolist() if c.dtype.kind == "S" else c.tolist() for c in cols]
+        return list(zip(*cols)), acc, codes
 
     def _kind_retry(self, st):
         """True when the scan is to be repeated with other key or value kinds (JSON scans)"""
@@ -996,11 +1016,12 @@ def _append_keys(keys, new):
 def _merge_fold_cols(keys, cols, extra, binop):
     """(keys, value columns) of a device fold plus {key: value} folded on the host: a key present in both gets
     binop(device value, host value). The columns are one int64 or float64 column, or mean()'s (sum, count) pairs
-    (int64 or float64 sums, int64 counts); `keys` is an 'S' array, an int64 array or a list of str. An int64 column
-    must hold every host-folded value as well as every merged one."""
+    (int64 or float64 sums, int64 counts); `keys` is an 'S' array, an int64 array, or a list of str or of tuples of
+    str and int. An int64 column must hold every host-folded value as well as every merged one, and every int key or
+    key component must be an int64."""
     if not extra:
         return keys, cols
-    if any(type(k) is int and not -(1 << 63) <= k < (1 << 63) for k in extra):
+    if any(type(c) is int and not -(1 << 63) <= c < (1 << 63) for k in extra for c in (k if type(k) is tuple else (k,))):
         raise NotLowerable("a host-folded key outside int64")
     cols = [np.array(c, copy=True) for c in cols]
 
@@ -1019,7 +1040,8 @@ def _merge_fold_cols(keys, cols, extra, binop):
     pos = _key_positions(keys, extra)
     new = []
     for k, v in extra.items():
-        i = pos.get(k) if type(k) in (str, int) else None
+        i = pos.get(k) if type(k) in (str, int) or (type(k) is tuple and all(type(c) in (str, int) for c in k)) \
+            else None
         if i is None:
             new.append(k)
             continue
@@ -1094,11 +1116,16 @@ def _match_text_count(stage, inputs):
     return src, mode
 
 
+KEY_TUPLE = "tuple"   # the key kind of a field scan's spec whose key is a tuple of fields
+
+
 def _match_text_fields(stage, inputs):
     """filter* [map(l.split(S) | l.split()) filter*] keyed(field key, 1 | int(field) | float(field)) +
     PartialReduceCombiner(+ | min | max), or mean()'s keyed(field key, (int(field) | float(field), 1)) + component-wise
     (+, +), over text, each filter one lowering.field_predicate on the key's separator: (sources, (sep byte or
-    FIELD_SEP_WS, key index, key kind, value index or FIELD_VAL_ONE), op, mean, device predicates) or None"""
+    FIELD_SEP_WS, key index, key kind, value index or FIELD_VAL_ONE), op, mean, device predicates) or None. A tuple
+    key of field projections has key kind KEY_TUPLE and, as its key index, the components ((index, FIELD_KEY_STR |
+    FIELD_KEY_INT), ...)."""
     if not isinstance(stage, GMap) or len(inputs) != 1:
         return None
     src = _text_files(inputs[0])
@@ -1113,10 +1140,13 @@ def _match_text_fields(stage, inputs):
         return None
     keyed = ks[-1][1]
     at = kinds.index("map") if "map" in kinds else None
-    spec = lowering.text_fields_spec(keyed.fn, keyed.fn2, ks[at][1].fn if at is not None else None, whitespace=True)
+    spec = lowering.text_fields_spec(keyed.fn, keyed.fn2, ks[at][1].fn if at is not None else None, whitespace=True,
+                                     tuple_keys=True)
     if spec is None:
         return None
     sep, ki, kkind, vi, vkind, mean = spec
+    if kkind == lowering.FIELD_TUPLE:
+        ki = tuple((i, dev.FIELD_KEY_INT if k == lowering.FIELD_INT else dev.FIELD_KEY_STR) for i, k in ki)
     preds = []
     for i, (k, o) in enumerate(ks[:-1]):
         if k == "filter":
@@ -1138,6 +1168,7 @@ def _match_text_fields(stage, inputs):
             return None
         op = (_FOLD_OPS_F64 if vkind == lowering.FIELD_FLOAT else _FOLD_OPS)[kind]
     return src, (dev.FIELD_SEP_WS if sep == lowering.SEP_WS else ord(sep), ki,
+                 KEY_TUPLE if kkind == lowering.FIELD_TUPLE else
                  dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR,
                  dev.FIELD_VAL_ONE if vi is None else vi), op, mean, tuple(preds)
 
@@ -1299,6 +1330,8 @@ def _lower_map(runner, stage, inputs, si):
             detail += " filtered=%d" % scan.filtered
         if spec[0] == dev.FIELD_SEP_WS:
             detail += " sep=ws"
+        if spec[2] == KEY_TUPLE:
+            detail += " key=tuple%d" % len(spec[1])
         runner.stats.add(stage, "device text fields scan+combine", detail)
         return Frame(scan.keys, [scan.values], scalar=True, combined=True)
     m = _match_json_fields(stage, inputs)

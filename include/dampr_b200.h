@@ -273,6 +273,41 @@ int32_t dampr_text_fields(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uin
  * Three kernels per range: a line count per 16 KB tile, one CTA's scan of the counts, the fold. */
 int32_t dampr_text_fields_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
                                   uint64_t own_hi, const dampr_fields_spec *spec, dampr_kv *rec);
+/* ---- tuple keys: `(l.split(S)[i], int(l.split(S)[j]), ...)`, GROUP BY of 1 .. DAMPR_FIELD_KEYS_MAX fields ----------
+ * The same folds, predicates, line rules and stats as dampr_text_fields / dampr_text_fields_records, with the key
+ * made of the components of `keys` instead of spec->key_field / spec->key_kind (neither is read). spec->sep is a
+ * separator byte or DAMPR_FIELD_SEP_WS (DAMPR_FIELD_SEP_JSON returns DAMPR_ERR_ARG, as does n outside 1 .. 4). A
+ * line is taken only when every component exists and every INT component is [+-]?[0-9]{1,18}.
+ * - Key code: the two running states of the field keys' seeded hash are fed, in order, the bytes of each STR
+ *   component, the 8 little-endian bytes of v ^ 2^63 of each INT component v, and one 0xFF byte between two
+ *   components (it never occurs in a taken line); the code is mix64(state ^ L * 0x9E3779B97F4A7C15) | 2^63 with L
+ *   the number of bytes fed, as for a hashed field key. Component kinds are fixed per call, so the bytes fed name
+ *   the tuple. No code is 0.
+ * - Representative: the LINE, (offset << 20) | length, the lowest-offset taken line of each entry. Every later
+ *   insert of another line re-splits the representative line (in global memory, same rules) and compares its
+ *   components with its own: STR as bytes, INT as parsed values. A mismatch sets DAMPR_TF_COLLISION. stats[5]
+ *   (hashed str keys) stays 0.
+ * dampr_table_fetch_words does not decode these tables: dampr_table_fetch_field_keys does. */
+#define DAMPR_FIELD_KEYS_MAX 4
+typedef struct dampr_field_keys {
+    int32_t n;                              /* components: 1 .. DAMPR_FIELD_KEYS_MAX                            */
+    int32_t field[DAMPR_FIELD_KEYS_MAX];    /* i of line.split(sep)[i]; negative counts from the end            */
+    int32_t kind[DAMPR_FIELD_KEYS_MAX];     /* DAMPR_FIELD_KEY_STR | DAMPR_FIELD_KEY_INT                        */
+} dampr_field_keys;
+int32_t dampr_text_fields_tuple(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo, uint64_t own_hi,
+                                const dampr_fields_spec *spec, const dampr_field_keys *keys);
+int32_t dampr_text_fields_tuple_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
+                                        uint64_t own_hi, const dampr_fields_spec *spec, const dampr_field_keys *keys,
+                                        dampr_kv *rec);
+/* decode a tuple-key table ON THE DEVICE: each entry's representative line is split again (sep and keys as in the
+ * scan) into one column per component. Two phases: cols == NULL sets *n (entries) and widths[j] (the longest STR
+ * component j, 0 for INT components) only. Then cols[j] = uint8[*n * widths[j]] (STR: NUL-padded, widths[j] >= 1,
+ * a longer component is cut at widths[j]) or int64[*n] (INT), counts[i] the accumulator and codes[i] the key code
+ * of row i (either may be NULL). Rows are in one unspecified order shared by every column. */
+int32_t dampr_table_fetch_field_keys(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, int32_t sep,
+                                     const dampr_field_keys *keys, uint32_t widths[DAMPR_FIELD_KEYS_MAX],
+                                     void *const cols[DAMPR_FIELD_KEYS_MAX], uint64_t *counts, uint64_t *codes,
+                                     uint64_t cap, uint64_t *n);
 /* ---- JSON-lines fold: `Dampr.json(path)` (map(json.loads)) with r["k"] keys and r["v"] / int(r["v"]) /
  *      float(r["v"]) values, and filters on r["m"] -------------------------------------------------------------------
  * The same folds as dampr_text_fields / dampr_text_fields_records with spec->sep = DAMPR_FIELD_SEP_JSON (the field

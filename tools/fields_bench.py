@@ -7,7 +7,7 @@ page-cache-warm file, the host-map MB/s on a sample, and whether the device and 
 
     python tools/fields_bench.py [--gb 2] [--keys 1000000] [--reps 3] [--sample-mb 32] [--out DIR]
                                  [--value int|float] [--op sum|min|max|mean] [--where none|str|int|float|set]
-                                 [--sep comma|ws]
+                                 [--sep comma|ws] [--key-fields 1|2|3]
 
 --value float writes the value field as float text (even lines "%.6f", odd lines repr() of the double, right-aligned
 in a 24-byte field) and folds float(r[2]); --op picks `+` (fold_by), min / max (a_group_by().reduce) or mean(). A run
@@ -26,6 +26,13 @@ MB/s, the stats line with filtered=N, and whether the host-map sample of the fil
 --sep ws writes the same rows with their fields joined by runs of 1-3 spaces or tabs instead of commas, a blank in
 front of about a quarter of them and behind another quarter (the filler field gives up the bytes, so every line keeps
 its LINE bytes), and runs the same pipelines with `l.split()`. The JSON line then also holds "sep": "ws".
+
+--key-fields 2 groups by the tuple (r[0], r[1]) and 3 by (r[0], r[1], r[-3]) (the key field again, counted from
+the end). The filler field then holds one of two strings (a lowercase run with 'a' or 'b' in its middle), so a tuple
+key has about twice as many groups as the single key (under --sep ws the filler's length also varies with the blank
+runs around it, which multiplies the groups; "distinct_keys" says how many). It works with every other option of the CSV rows, and the JSON
+line also holds "key_fields" and "fetch_to_frame_ms" (the time from the table fetch to the key column of Python
+tuples, best run).
 
 --format json writes JSON lines of JLINE bytes instead: {"user": "u%07d", "n": int, "status": an int or a string,
 "latency": float, "meta": {"user": "decoy", ...}, "pad": filler}, padded with JSON whitespace after the numbers, and
@@ -161,6 +168,24 @@ WHERE = {"str": lambda r: r[0] < "u0500000", "int": lambda r: int(r[2]) >= 0, "f
          "set": lambda r: r[0] not in SET_KEYS}
 
 
+def rewrite_filler(text, seed, key_fields):
+    """--key-fields 2 and 3: the filler field of every row becomes one of two strings ('f' letters with 'a' or 'b' at
+    byte 50, which lies inside the filler of both layouts and is not touched by whitespace_rows)"""
+    if key_fields > 1:
+        rows = text.reshape(-1, LINE)
+        rng = np.random.default_rng(seed)
+        step = 1 << 20
+        for a in range(0, len(rows), step):
+            t = rows[a:a + step]
+            fill_end = 92 if t[0, 92] == ord(",") else LINE - 2 - FVAL
+            t[:, 9:fill_end] = ord("f")
+            t[:, 50] = ord("a") + rng.integers(0, 2, size=len(t), dtype=np.uint8)
+    return text
+
+
+KEY_FNS = {1: lambda r: r[0], 2: lambda r: (r[0], r[1]), 3: lambda r: (r[0], r[1], r[-3])}
+
+
 def splitter(sep):
     return (lambda l: l.split()) if sep == "ws" else (lambda l: l.split(","))
 
@@ -183,30 +208,32 @@ def json_rows(sample, value):
         yield r["user"], (r["n"] if value == "int" else float(r["latency"]))
 
 
-def job(Dampr, src, value="int", op="sum", where="none", sep="comma"):
+def job(Dampr, src, value="int", op="sum", where="none", sep="comma", key_fields=1):
     if sep == "json":
         return json_job(Dampr, src, value, op)
     conv = int if value == "int" else float
+    key = KEY_FNS[key_fields]
     d = Dampr.read_input(src).map(splitter(sep))
     if where != "none":
         d = d.filter(WHERE[where])
     if op == "mean":
-        return d.mean(lambda r: r[0], lambda r: conv(r[2]))
+        return d.mean(key, lambda r: conv(r[2]))
     if op in ("min", "max"):
-        return d.a_group_by(lambda r: r[0], lambda r: conv(r[2])).reduce(min if op == "min" else max)
-    return d.fold_by(lambda r: r[0], value=lambda r: conv(r[2]), binop=lambda a, b: a + b)
+        return d.a_group_by(key, lambda r: conv(r[2])).reduce(min if op == "min" else max)
+    return d.fold_by(key, value=lambda r: conv(r[2]), binop=lambda a, b: a + b)
 
 
-def python_fold(sample, value, op, where="none", sep="comma"):
+def python_fold(sample, value, op, where="none", sep="comma", key_fields=1):
     """the stage as plain Python over the sample's lines: {key: result}"""
     conv = int if value == "int" else float
     keep = WHERE.get(where, lambda r: True)
     split = splitter(sep)
+    key = KEY_FNS[key_fields]
     out = {}
     if sep == "json":
         rows = json_rows(sample, value)
     else:
-        rows = ((r[0], conv(r[2])) for r in map(split, sample.decode("ascii").split("\n")[:-1]) if keep(r))
+        rows = ((key(r), conv(r[2])) for r in map(split, sample.decode("ascii").split("\n")[:-1]) if keep(r))
     for k, v in rows:
         if op == "mean":
             s, n = out.get(k, (0, 0))
@@ -220,12 +247,13 @@ def python_fold(sample, value, op, where="none", sep="comma"):
     return out
 
 
-def magnitudes(sample, sep="comma"):
+def magnitudes(sample, sep="comma", key_fields=1):
     """{key: (lines, sum of |float value|)} of the sample: the scale of the sum bound"""
     mag = {}
     split = splitter(sep)
+    key = KEY_FNS[key_fields]
     rows = json_rows(sample, "float") if sep == "json" else \
-        ((r[0], r[2]) for r in map(split, sample.decode("ascii").split("\n")[:-1]))
+        ((key(r), r[2]) for r in map(split, sample.decode("ascii").split("\n")[:-1]))
     for k, v in rows:
         n, a = mag.get(k, (0, 0.0))
         mag[k] = (n + 1, a + abs(float(v)))
@@ -267,16 +295,18 @@ def main():
     ap.add_argument("--where", choices=("none", "str", "int", "float", "set"), default="none")
     ap.add_argument("--sep", choices=("comma", "ws", ","), default="comma")
     ap.add_argument("--format", choices=("csv", "json"), default="csv")
+    ap.add_argument("--key-fields", type=int, choices=(1, 2, 3), default=1)
     a = ap.parse_args()
     if a.sep == ",":
         a.sep = "comma"
     if a.format == "json":
-        if a.where != "none" or a.sep != "comma":
-            ap.error("--format json takes neither --where nor --sep")
+        if a.where != "none" or a.sep != "comma" or a.key_fields != 1:
+            ap.error("--format json takes neither --where, --sep nor --key-fields")
         a.sep = "json"
     if a.where == "int" and a.value != "int":
         ap.error("--where int needs --value int (int() of a float field raises)")
-    default = a.value == "int" and a.op == "sum"
+    default = a.value == "int" and a.op == "sum" and a.key_fields == 1
+    K = a.key_fields
 
     from dampr_b200 import Dampr, device as dev, plan
     from dampr_b200 import runner as runner_mod
@@ -288,6 +318,7 @@ def main():
         text = json_text(2026, n_lines, a.keys)
     else:
         text = csv_text(2026, n_lines, a.keys) if a.value == "int" else float_text(2026, n_lines, a.keys)
+        text = rewrite_filler(text, 2028, K)
     if a.sep == "ws":
         text = whitespace_rows(text, 2027, 6 if a.value == "int" else FVAL)
     nbytes = len(text)
@@ -298,10 +329,21 @@ def main():
     text.tofile(path)
     del text
 
+    fetch_s = []   # --key-fields: seconds from the table fetch to the list of key tuples, per scan
+    if K > 1:
+        fetch = plan.FieldScan._fetch_tuple_keys
+
+        def timed_fetch(scan, tab, tb):
+            t = time.perf_counter()
+            out = fetch(scan, tab, tb)
+            fetch_s.append(time.perf_counter() - t)
+            return out
+        plan.FieldScan._fetch_tuple_keys = timed_fetch
+
     def timed(src, where="none"):
         ctx.timings_reset()
         t0 = time.perf_counter()
-        n = len(list(job(Dampr, src, a.value, a.op, where, a.sep).run()))
+        n = len(list(job(Dampr, src, a.value, a.op, where, a.sep, K).run()))
         dt = time.perf_counter() - t0
         stages = runner_mod.LAST_STATS.stages
         assert "device text fields scan+combine" in stages[0][1], stages
@@ -338,11 +380,11 @@ def main():
             k, v = r[0], int(r[2])
             host[k] = host[k] + v if k in host else v
     else:
-        host = python_fold(sample, a.value, a.op, sep=a.sep)
+        host = python_fold(sample, a.value, a.op, sep=a.sep, key_fields=K)
     host_s = time.perf_counter() - t0
     spin = dev.PinnedBuffer(len(sample))
     spin.array[:] = np.frombuffer(sample, dtype=np.uint8)
-    got = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op, sep=a.sep).run())
+    got = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op, sep=a.sep, key_fields=K).run())
 
     kernel_ms = min(m[1] for m in mem)
     res = {
@@ -367,12 +409,14 @@ def main():
         res.update({"value": a.value, "op": a.op,
                     "kernels_ms": {k: round(v, 3) for k, v in sorted(best[4].items())}})
         if a.value == "float" and a.op in ("sum", "mean"):
-            res["sample_within_bound"] = within_bound(got, host, magnitudes(sample, a.sep), a.op)
+            res["sample_within_bound"] = within_bound(got, host, magnitudes(sample, a.sep, K), a.op)
+    if K > 1:
+        res.update({"key_fields": K, "fetch_to_frame_ms": round(1e3 * min(fetch_s[1:1 + a.reps]), 3)})
     if a.where != "none":
         t0 = time.perf_counter()
-        whost = python_fold(sample, a.value, a.op, a.where, a.sep)
+        whost = python_fold(sample, a.value, a.op, a.where, a.sep, K)
         whost_s = time.perf_counter() - t0
-        wgot = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op, a.where, a.sep).run())
+        wgot = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op, a.where, a.sep, K).run())
         wk = min(m[1] for m in wmem)
         res.update({
             "where": a.where,
@@ -383,7 +427,7 @@ def main():
             "where_e2e_file_warm_MBps": round(nbytes / min(f[0] for f in wfil) / 1e6, 1),
             "where_host_map_MBps": round(len(sample) / whost_s / 1e6, 1),
             "where_sample_equal": wgot == whost if not (a.value == "float" and a.op in ("sum", "mean")) else
-            within_bound(wgot, whost, magnitudes(sample, a.sep), a.op),
+            within_bound(wgot, whost, magnitudes(sample, a.sep, K), a.op),
             "where_stats": wmem[0][3],
         })
     if a.sep == "ws":
