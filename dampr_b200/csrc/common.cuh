@@ -18,6 +18,27 @@ typedef uint8_t u8;
 
 #define DAMPR_NUM_SMS_DEFAULT 132
 
+// Opcodes of the numeric expression programs (lowering.numeric_program): one int32 per operation, opcode in the low
+// byte, argument above it. Postfix over a typed stack of int64 ("int") and double ("float") values, typed as CPython
+// types the expression. dampr_host_eval_f64 evaluates EV_X .. EV_FNEG; the field scans' programs (dampr_field_expr)
+// take every opcode but EV_X and EV_LOG.
+enum EvalOp : int32_t {
+    EV_X = 0,      // push the column value (int)
+    EV_CI = 1,     // push int constant ci[arg]
+    EV_CF = 2,     // push float constant cf[arg]
+    EV_I2F = 3,    // float() of the int on top
+    EV_IADD = 4, EV_ISUB = 5, EV_IMUL = 6,
+    EV_FADD = 7, EV_FSUB = 8, EV_FMUL = 9, EV_FDIV = 10,
+    EV_IDIV = 11,  // int / int: true division
+    EV_LOG = 12,   // math.log of the float on top
+    EV_INEG = 13, EV_FNEG = 14,
+    EV_LOAD = 15,  // push load slot arg (its kind gives the type: int(), float() or len() of a field)
+    EV_NF = 16,    // push the line's field count, len(line.split(sep)) (int)
+    EV_IFLOOR = 17, EV_IMOD = 18,  // int // int and int % int, floored as in CPython
+    EV_IABS = 19, EV_FABS = 20,
+    EV_F2I = 21,   // int() of the float on top (truncation)
+};
+
 struct TimedKernel {
     int id;
     cudaEvent_t beg, end;

@@ -461,6 +461,180 @@ struct TupleWhere {
     TupleView tup;
 };
 
+// ---- computed keys and values ----------------------------------------------------------------------------------
+constexpr int X_OPS = DAMPR_EXPR_MAX_OPS;
+constexpr int X_DEPTH = DAMPR_EXPR_MAX_DEPTH;
+constexpr int X_CONSTS = DAMPR_EXPR_MAX_CONSTS;
+constexpr long long X_I64_MIN = (long long)0x8000000000000000ULL, X_I64_MAX = 0x7FFFFFFFFFFFFFFFLL;
+static_assert(DAMPR_EXPR_MAX_LOADS == T_MAX, "load slots take the tuple components' bound slots");
+
+// the programs of an expression scan (checked on the host: every operand is there and of its type), passed by value
+// in the kernel parameters; the load slots' fields are the TupleView's
+struct ExprView {
+    int key_len, val_len;   // 0: the spec's key / value
+    int key_prog[X_OPS], val_prog[X_OPS];
+    long long ci[X_CONSTS];
+    double cf[X_CONSTS];
+    int load_kind[T_MAX];
+};
+
+// the parameters of an expression build: fields_tiles finds `tup` (the load slots) where a tuple build does, and `ex`
+// behind it
+struct ExprWhere {
+    WhereView where;
+    TupleView tup;
+    ExprView ex;
+};
+
+// the value of load slot j (unrolled: the slots stay in registers)
+__device__ __forceinline__ long long load_slot(const long long (&lv)[T_MAX], int j) {
+    long long v = 0;
+#pragma unroll
+    for (int i = 0; i < T_MAX; ++i)
+        if (i == j) v = lv[i];
+    return v;
+}
+
+__device__ __forceinline__ double as_f(long long x) { return __longlong_as_double(x); }
+__device__ __forceinline__ long long as_i(double x) { return __double_as_longlong(x); }
+
+// run one program over the line's loads lv and field count nf: false where CPython raises or leaves int64 (the line
+// is the host's); out holds an int64 or the bits of a double. Every float operation is one IEEE rounding (the
+// intrinsics keep ptxas from contracting a * b + c).
+__device__ __noinline__ bool eval_expr(const ExprView &ex, const int *prog, int len, long long l0, long long l1,
+                                       long long l2, long long l3, int nf, long long &out) {
+    const long long lv[T_MAX] = {l0, l1, l2, l3};
+    constexpr long long LIM53 = 1LL << 53;
+    long long st[X_DEPTH];
+    int sp = 0;
+    for (int pc = 0; pc < len; ++pc) {
+        const int w = prog[pc], op = w & 0xFF, arg = w >> 8;
+        if (op == EV_CI || op == EV_CF || op == EV_LOAD || op == EV_NF) {
+            st[sp++] = op == EV_CI ? ex.ci[arg] : op == EV_CF ? as_i(ex.cf[arg]) : op == EV_LOAD ? load_slot(lv, arg)
+                                                                                                : (long long)nf;
+            continue;
+        }
+        long long &b = st[sp - 1];
+        switch (op) {   // unary operations
+            case EV_I2F: b = as_i(__ll2double_rn(b)); continue;
+            case EV_INEG:
+                if (b == X_I64_MIN) return false;
+                b = -b;
+                continue;
+            case EV_IABS:
+                if (b == X_I64_MIN) return false;
+                b = b < 0 ? -b : b;
+                continue;
+            case EV_FNEG: b ^= X_I64_MIN; continue;
+            case EV_FABS: b &= X_I64_MAX; continue;
+            case EV_F2I: {   // int(x): a NaN or an infinity raises, a float outside int64 is a big int
+                const double x = as_f(b);
+                if (!(x >= -9223372036854775808.0 && x < 9223372036854775808.0)) return false;
+                b = __double2ll_rz(x);
+                continue;
+            }
+            default: break;
+        }
+        long long &a = st[sp - 2];
+        --sp;
+        switch (op) {
+            case EV_IADD: {
+                const long long r = (long long)((u64)a + (u64)b);
+                if (((a ^ r) & (b ^ r)) < 0) return false;
+                a = r;
+                break;
+            }
+            case EV_ISUB: {
+                const long long r = (long long)((u64)a - (u64)b);
+                if (((a ^ b) & (a ^ r)) < 0) return false;
+                a = r;
+                break;
+            }
+            case EV_IMUL: {
+                const long long lo = (long long)((u64)a * (u64)b);
+                if (__mul64hi(a, b) != (lo >> 63)) return false;
+                a = lo;
+                break;
+            }
+            case EV_IDIV:   // int / int: CPython divides the doubles when both operands are within 2^53
+                if (b == 0 || a > LIM53 || a < -LIM53 || b > LIM53 || b < -LIM53) return false;
+                a = as_i(__ddiv_rn(__ll2double_rn(a), __ll2double_rn(b)));
+                break;
+            case EV_IFLOOR: {
+                if (b == 0 || (a == X_I64_MIN && b == -1)) return false;
+                long long q = a / b;
+                if (q * b != a && ((a < 0) != (b < 0))) --q;
+                a = q;
+                break;
+            }
+            case EV_IMOD: {
+                if (b == 0) return false;
+                long long r = b == -1 ? 0 : a % b;
+                if (r != 0 && ((r < 0) != (b < 0))) r += b;
+                a = r;
+                break;
+            }
+            case EV_FADD: a = as_i(__dadd_rn(as_f(a), as_f(b))); break;
+            case EV_FSUB: a = as_i(__dsub_rn(as_f(a), as_f(b))); break;
+            case EV_FMUL: a = as_i(__dmul_rn(as_f(a), as_f(b))); break;
+            default:   // EV_FDIV
+                if (as_f(b) == 0.0) return false;
+                a = as_i(__ddiv_rn(as_f(a), as_f(b)));
+                break;
+        }
+    }
+    out = st[0];
+    return true;
+}
+
+// a CTA's hot-key slots of an expression scan with a key program: key codes and their accumulators in the table's
+// encoding, folded with shared-memory atomics and inserted into the table once, after the CTA's last tile
+constexpr int X_HOT = 32;
+struct HotKeys {
+    u64 code[X_HOT];
+    u64 acc[X_HOT];
+};
+
+__device__ __forceinline__ HotKeys &hot_keys() {
+    __shared__ HotKeys h;
+    return h;
+}
+
+// the table's accumulator encoding of one value under op (see the header): SUM the value, MAX / MIN order codes
+__device__ __forceinline__ u64 table_code(int op, long long v) {
+    if (op == DAMPR_OP_SUM_I64) return (u64)v;
+    const u64 ord = op == DAMPR_OP_MIN_F64 || op == DAMPR_OP_MAX_F64
+                        ? (u64)v ^ (v < 0 ? ~0ULL : 0x8000000000000000ULL)
+                        : (u64)v ^ 0x8000000000000000ULL;
+    return op == DAMPR_OP_MAX_I64 || op == DAMPR_OP_MAX_F64 ? ord : ~ord;
+}
+
+__device__ __forceinline__ void fold_code(u64 *acc, int op, u64 c) {
+    if (op == DAMPR_OP_SUM_I64) atomicAdd(acc, c);
+    else atomicMax(acc, c);
+}
+
+// fold an encoded accumulator c of an int key code into the table
+__device__ __forceinline__ void table_fold_code(const FieldsView &t, u64 code, u64 c, u32 &flags) {
+    u64 slot = mix64(code) & t.mask;
+    for (u32 probe = 0; probe < F_G_MAX_PROBES; ++probe) {
+        u64 k = *((volatile u64 *)&t.keys[slot]);
+        if (k == 0) {
+            k = atomicCAS(&t.keys[slot], 0ULL, code);
+            if (k == 0) {
+                atomicAdd(&t.stats[S_ENTRIES], 1ULL);
+                k = code;
+            }
+        }
+        if (k == code) {
+            fold_code(&t.counts[slot], t.op, c);
+            return;
+        }
+        slot = (slot + 1) & t.mask;
+    }
+    flags |= DAMPR_TF_TABLEFULL;
+}
+
 // a tuple-key line's components: field ci[j] (-1: no component j, or it is missing: `missing`), bounds
 // [cs[j], ce[j]) in the window; nothing in the other builds
 template <bool TUP>
@@ -641,6 +815,65 @@ __device__ __forceinline__ void put_record(const RecView &rv, u64 ix, u64 code, 
     else flags |= DAMPR_TF_RECFULL;
 }
 
+// an expression scan's key and value of a line that passed its predicates (every field bound found): the load slots
+// parsed, then the programs run, or the spec's key and value read as the plain scan reads them (g0: the global offset
+// of window position 0). false when the line is the host's: a missing slot field (IndexError), a slot the device does
+// not parse, or a program that does not reach CPython's result.
+template <int VK>
+__device__ __forceinline__ bool expr_line(const u8 *t, const TupleBounds<true> &kb, const TupleView &tv,
+                                          const ExprView &ex, bool kx, bool vx, int nf, const FieldsView &tab, u32 ks,
+                                          u32 ke, u32 vs, u32 ve, u64 g0, long long &val, u64 &code, u64 &rep,
+                                          u64 &acc_long, u32 &flags) {
+    if (kb.missing) return false;
+    long long lv[T_MAX];
+#pragma unroll
+    for (int j = 0; j < T_MAX; ++j) {
+        lv[j] = 0;
+        if (j < tv.n) {
+            const u8 *p = t + kb.cs[j];
+            const u32 len = kb.ce[j] - kb.cs[j];
+            if (ex.load_kind[j] == DAMPR_LOAD_LEN) {
+                lv[j] = len;
+            } else if (ex.load_kind[j] == DAMPR_LOAD_INT) {
+                if (!parse_int(p, len, lv[j])) return false;
+            } else {
+                double d;
+                if (!parse_f64(p, len, d)) return false;
+                lv[j] = as_i(d);
+            }
+        }
+    }
+    if (vx) {
+        if (!eval_expr(ex, ex.val_prog, ex.val_len, lv[0], lv[1], lv[2], lv[3], nf, val)) return false;
+    } else if constexpr (VK == VK_F64) {
+        double d;
+        if (!parse_f64(t + vs, ve - vs, d)) return false;
+        val = as_i(d);
+    } else if (tab.val_field != DAMPR_FIELD_VAL_ONE) {
+        if (!parse_int(t + vs, ve - vs, val)) return false;
+    }
+    if (kx) {   // INT64_MIN would code to 0, the empty slot
+        long long k;
+        if (!eval_expr(ex, ex.key_prog, ex.key_len, lv[0], lv[1], lv[2], lv[3], nf, k) || k == X_I64_MIN) return false;
+        code = (u64)k ^ 0x8000000000000000ULL;
+    } else if (tab.key_int) {
+        long long k;
+        if (!parse_int(t + ks, ke - ks, k)) return false;
+        code = (u64)k ^ 0x8000000000000000ULL;
+    } else {
+        const u32 klen = ke - ks;
+        if (klen >= 1 && klen <= 9) {
+            for (int i = (int)klen - 1; i >= 0; --i) code = (code << 7) | t[ks + i];
+        } else {
+            code = hash_bytes(t + ks, klen, tab.seed);
+            rep = ((g0 + ks) << 20) | klen;
+            acc_long++;
+        }
+    }
+    if (VK == VK_F64 && vx && isnan(as_f(val))) flags |= DAMPR_TF_NAN;
+    return true;
+}
+
 // lines per tile -> record index of each tile's first line (exclusive scan from the running count, which
 // advances by the range's lines): one CTA, no inter-CTA waiting
 __global__ void __launch_bounds__(SCAN_THREADS) fields_tile_scan_kernel(u64 *tiles, u64 ntiles, u64 *run) {
@@ -768,8 +1001,9 @@ __device__ __forceinline__ void json_fold(const u8 *t, u32 q, u32 end, u64 g0, c
 // the kernel body over the tiles of [own_lo, own_hi); where: the predicates of a WHERE scan; WS: split on runs of
 // whitespace (`line.split()`) instead of the separator byte; JSON: json.loads each line and read the members *json;
 // TUP: the key is the tuple of the components that follow the predicates (where points into a TupleWhere;
-// tab.key_field is component 0's field, tab.key_int is not read)
-template <int VK, int MODE, bool WHERE, bool WS, bool JSON = false, bool TUP = false>
+// tab.key_field is component 0's field, tab.key_int is not read); EXPR: the load slots follow the predicates as TUP's
+// components do, and the programs follow them (where points into an ExprWhere)
+template <int VK, int MODE, bool WHERE, bool WS, bool JSON = false, bool TUP = false, bool EXPR = false>
 __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi,
                                              const FieldsView &tab, const RecView &rv, const WhereView *where,
                                              const JsonView *json = nullptr) {
@@ -779,6 +1013,10 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
     const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
     const bool cr_data = tab.cr_is_data != 0;
     if (tid == 0) s.flags = 0;
+    if constexpr (EXPR) {   // (the first tile's __syncthreads orders this before any fold)
+        HotKeys &h = hot_keys();
+        if (tid < X_HOT) h.code[tid] = h.acc[tid] = 0;
+    }
 
     u64 acc_lines = 0, acc_long = 0, acc_maxabs = 0;
     u64 acc_dropped = 0;   // WHERE: lines a predicate rejected
@@ -901,19 +1139,22 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
             bool dropped = false;   // WHERE: a predicate is false
             long long val = 1, kval = 0;
             u64 code = 0, rep = ~0ULL;
-            TupleBounds<TUP> kb;   // TUP: the key components' fields and bounds
-            const TupleView *tup = TUP ? &reinterpret_cast<const TupleWhere *>(where)->tup : nullptr;
+            TupleBounds<TUP || EXPR> kb;   // TUP: the key components' fields and bounds; EXPR: the load slots'
+            const TupleView *tup = TUP || EXPR ? &reinterpret_cast<const TupleWhere *>(where)->tup : nullptr;
+            const ExprView *ex = EXPR ? &reinterpret_cast<const ExprWhere *>(where)->ex : nullptr;
+            const bool kx = EXPR && ex->key_len > 0, vx = EXPR && ex->val_len > 0;   // a computed key / value
             if constexpr (JSON) {
                 if (!to_host) json_fold<VK, WHERE>(s.text, q, end, gq - q, tab, *json, where, to_host, dropped, val, code,
                                                    rep, acc_long, my_flags);
             } else if (!to_host) {
                 // resolve the field indices (Python semantics: negative counts from the end)
                 const int nf = WS ? (int)nsep : (int)nsep + 1;
-                const int ki = tab.key_field < 0 ? tab.key_field + nf : tab.key_field;
-                const bool one = tab.val_field == DAMPR_FIELD_VAL_ONE;
+                const int ki = kx ? 0 : tab.key_field < 0 ? tab.key_field + nf : tab.key_field;
+                const bool one = vx || tab.val_field == DAMPR_FIELD_VAL_ONE;
                 const int vi = one ? 0 : (tab.val_field < 0 ? tab.val_field + nf : tab.val_field);
-                const bool kv_missing = ki < 0 || ki >= nf || vi < 0 || vi >= nf;
-                if constexpr (TUP) {   // (tab.key_field is component 0's field: kv_missing covers it)
+                const bool kv_missing = EXPR ? (!kx && (ki < 0 || ki >= nf)) || (!one && (vi < 0 || vi >= nf))
+                                             : ki < 0 || ki >= nf || vi < 0 || vi >= nf;
+                if constexpr (TUP || EXPR) {   // (tab.key_field is component 0's field: kv_missing covers it)
 #pragma unroll
                     for (int j = 0; j < T_MAX; ++j) {
                         int i = -1;
@@ -955,7 +1196,7 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                             need = max(need, pi[j] + 1);
                         }
                     }
-                    if constexpr (TUP) {
+                    if constexpr (TUP || EXPR) {
 #pragma unroll
                         for (int j = 0; j < T_MAX; ++j) need = max(need, kb.ci[j] + 1);
                     }
@@ -988,7 +1229,7 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                                         for (int j = 0; j < P_MAX; ++j)
                                             if (fi == pi[j]) pe[j] = p;
                                     }
-                                    if constexpr (TUP) {
+                                    if constexpr (TUP || EXPR) {
 #pragma unroll
                                         for (int j = 0; j < T_MAX; ++j)
                                             if (fi == kb.ci[j]) kb.ce[j] = p;
@@ -1001,7 +1242,7 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                                         for (int j = 0; j < P_MAX; ++j)
                                             if (fi == pi[j]) ps[j] = p;
                                     }
-                                    if constexpr (TUP) {
+                                    if constexpr (TUP || EXPR) {
 #pragma unroll
                                         for (int j = 0; j < T_MAX; ++j)
                                             if (fi == kb.ci[j]) kb.cs[j] = p;
@@ -1030,7 +1271,7 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                                     for (int j = 0; j < P_MAX; ++j)
                                         if (f == pi[j]) pe[j] = p;
                                 }
-                                if constexpr (TUP) {
+                                if constexpr (TUP || EXPR) {
 #pragma unroll
                                     for (int j = 0; j < T_MAX; ++j)
                                         if (f == kb.ci[j]) kb.ce[j] = p;
@@ -1043,7 +1284,7 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                                     for (int j = 0; j < P_MAX; ++j)
                                         if (f == pi[j]) ps[j] = p + 1;
                                 }
-                                if constexpr (TUP) {
+                                if constexpr (TUP || EXPR) {
 #pragma unroll
                                     for (int j = 0; j < T_MAX; ++j)
                                         if (f == kb.ci[j]) kb.cs[j] = p + 1;
@@ -1063,7 +1304,11 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                         dropped = verdict == 0;
                         to_host = verdict < 0 || (verdict == 1 && kv_missing);
                     }
-                    if (!WHERE || !(to_host || dropped)) {
+                    if constexpr (EXPR) {
+                        if (!WHERE || !(to_host || dropped))
+                            to_host = !expr_line<VK>(s.text, kb, *tup, *ex, kx, vx, nf, tab, ks, ke, vs, ve,
+                                                     sgl - F_LEAD, val, code, rep, acc_long, my_flags);
+                    } else if (!WHERE || !(to_host || dropped)) {
                         const u32 klen = ke - ks;
                         if constexpr (VK == VK_F64) {
                             double d;
@@ -1129,7 +1374,24 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                 my_flags |= DAMPR_TF_NEGZERO;
             }
             bool same;
-            if constexpr (TUP) {
+            if constexpr (EXPR) {
+                // an int-expression key folds into the CTA's hot-key slots first (a constant key, or a few buckets,
+                // would otherwise send every line to one table slot); str keys keep one insert per line
+                if constexpr (MODE == M_RECORDS) put_record(rv, tbase + li, code, (u64)val, my_flags);
+                if (kx) {
+                    HotKeys &h = hot_keys();
+                    const u32 hs = (u32)mix64(code) & (X_HOT - 1);
+                    const u64 c = atomicCAS(&h.code[hs], 0ULL, code);
+                    const long long v = MODE == M_RECORDS ? 1 : val;
+                    if (c == 0 || c == code) fold_code(&h.acc[hs], tab.op, table_code(tab.op, v));
+                    else fold_insert<MODE != M_RECORDS && VK == VK_F64>(tab, text, code, v, rep, my_flags);
+                    same = true;
+                } else if constexpr (MODE == M_RECORDS) {
+                    same = fold_insert<false>(tab, text, code, 1, rep, my_flags);
+                } else {
+                    same = fold_insert<VK == VK_F64>(tab, text, code, val, rep, my_flags);
+                }
+            } else if constexpr (TUP) {
                 // the guard re-splits the entry's representative line when it is another one than this line
                 u64 other = ~0ULL;
                 if constexpr (MODE == M_RECORDS) {
@@ -1147,6 +1409,12 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
             }
             if (!same) my_flags |= DAMPR_TF_COLLISION;
         }
+    }
+
+    if constexpr (EXPR) {   // the hot-key slots into the table, one insert per slot
+        __syncthreads();
+        HotKeys &h = hot_keys();
+        if (tid < X_HOT && h.code[tid]) table_fold_code(tab, h.code[tid], h.acc[tid], my_flags);
     }
 
     // ---- publish counters ---------------------------------------------------------------------------------
@@ -1222,17 +1490,41 @@ text_fields_tuple_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own
 }
 static_assert(sizeof(TupleWhere) + 256 <= 4096, "kernel parameters");
 
+// the expression builds (plain and WHERE) of the separator-byte and whitespace scans: the load slots, the programs
+// (and the predicates, unused by a plain build) read in place from the parameters
+template <int VK, int MODE, bool WHERE, bool WS>
+__global__ void __launch_bounds__(F_THREADS, 4)
+text_fields_expr_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv,
+                        const __grid_constant__ ExprWhere xw) {
+    static_assert(MODE != M_COUNT, "the count pass is the plain kernel's");
+    fields_tiles<VK, MODE, WHERE, WS, false, false, true>(text, n, own_lo, own_hi, tab, rv, &xw.where);
+}
+static_assert(sizeof(ExprWhere) + 256 <= 4096, "kernel parameters");
+
 // one kernel over the tiles of [own_lo, own_hi); WHERE: the build that applies the predicates *wh; WS: the
-// whitespace-split build; JSON: the JSON-lines build over the members *jv; TUP: the tuple-key build over *tk
+// whitespace-split build; JSON: the JSON-lines build over the members *jv; TUP: the tuple-key build over *tk; xe: the
+// expression build over the load slots *tk and the programs *xe
 template <int VK, int MODE, bool WHERE = false, bool WS = false, bool JSON = false, bool TUP = false>
 int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const FieldsView &tv, const RecView &rv,
                   int timer, const WhereView *wh = nullptr, const JsonView *jv = nullptr,
-                  const TupleView *tk = nullptr) {
+                  const TupleView *tk = nullptr, const ExprView *xe = nullptr) {
     const size_t smem = sizeof(SmemF);
     const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
     u64 grid = (u64)ctx->num_sms * 4;
     if (grid > ntiles) grid = ntiles;
-    if constexpr (TUP) {
+    if (xe) {
+        if constexpr (!JSON && !TUP && MODE != M_COUNT) {
+            ExprWhere xw{};
+            if (wh) xw.where = *wh;
+            xw.tup = *tk;
+            xw.ex = *xe;
+            void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, ExprWhere) =
+                text_fields_expr_kernel<VK, MODE, WHERE, WS>;
+            CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            ScopedTimer tm(ctx, timer);
+            kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, xw);
+        }
+    } else if constexpr (TUP) {
         TupleWhere tw{};
         if (wh) tw.where = *wh;
         tw.tup = *tk;
@@ -1369,10 +1661,19 @@ FieldsView fields_view(dampr_table *t, const dampr_fields_spec *spec, int op) {
 }
 
 // the fold pass of one range under one separator class: the plain kernel, or its WHERE build when spec holds
-// predicates; tk: the tuple-key builds over those components
+// predicates; tk: the tuple-key builds over those components; xe: the expression builds over the load slots tk
 template <int VK, int MODE, bool WS>
 int launch_fold_sep(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
-                    const FieldsView &tv, const RecView &rv, const TupleView *tk) {
+                    const FieldsView &tv, const RecView &rv, const TupleView *tk, const ExprView *xe = nullptr) {
+    if (xe) {
+        WhereView w{};
+        if (spec->npreds == 0)
+            return launch_fields<VK, MODE, false, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, nullptr,
+                                                      nullptr, tk, xe);
+        if (int r = where_view(ctx, spec, w)) return r;
+        return launch_fields<VK, MODE, true, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w, nullptr,
+                                                 tk, xe);
+    }
     if (spec->npreds == 0) {
         if (!tk) return launch_fields<VK, MODE, false, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS);
         return launch_fields<VK, MODE, false, WS, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS,
@@ -1401,10 +1702,10 @@ int launch_json_fold(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, 
 // the fold pass of one range: the separator-byte build, or the whitespace-split one under DAMPR_FIELD_SEP_WS
 template <int VK, int MODE>
 int launch_fold(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
-                const FieldsView &tv, const RecView &rv, const TupleView *tk = nullptr) {
+                const FieldsView &tv, const RecView &rv, const TupleView *tk = nullptr, const ExprView *xe = nullptr) {
     if (spec->sep == DAMPR_FIELD_SEP_WS)
-        return launch_fold_sep<VK, MODE, true>(ctx, tb, own_lo, own_hi, spec, tv, rv, tk);
-    return launch_fold_sep<VK, MODE, false>(ctx, tb, own_lo, own_hi, spec, tv, rv, tk);
+        return launch_fold_sep<VK, MODE, true>(ctx, tb, own_lo, own_hi, spec, tv, rv, tk, xe);
+    return launch_fold_sep<VK, MODE, false>(ctx, tb, own_lo, own_hi, spec, tv, rv, tk, xe);
 }
 
 // the components of a tuple-key call in kernel-parameter form
@@ -1419,6 +1720,78 @@ int tuple_view(dampr_ctx *ctx, const dampr_field_keys *keys, TupleView &tk) {
         tk.field[j] = keys->field[j];
         tk.is_int[j] = keys->kind[j] == DAMPR_FIELD_KEY_INT;
     }
+    return DAMPR_OK;
+}
+
+// one program of an expression call, checked once: every operation finds operands of its type, the stack stays
+// within X_DEPTH and ends with one value of type want ('i' or 'f'); constants and load slots (kinds lk) in range
+bool expr_program_ok(const int32_t *prog, int len, char want, const int32_t *lk, int nloads) {
+    if (len < 1 || len > X_OPS) return false;
+    char st[X_DEPTH];
+    int sp = 0;
+    for (int pc = 0; pc < len; ++pc) {
+        const int op = prog[pc] & 0xFF, arg = prog[pc] >> 8;
+        char push = 0, in = 0, out = 0;   // a leaf's type, or an operation's operand and result types
+        int arity = 0;
+        switch (op) {
+            case EV_CI: push = arg >= 0 && arg < X_CONSTS ? 'i' : 0; break;
+            case EV_CF: push = arg >= 0 && arg < X_CONSTS ? 'f' : 0; break;
+            case EV_LOAD: push = arg >= 0 && arg < nloads ? (lk[arg] == DAMPR_LOAD_F64 ? 'f' : 'i') : 0; break;
+            case EV_NF: push = 'i'; break;
+            case EV_I2F: arity = 1, in = 'i', out = 'f'; break;
+            case EV_F2I: arity = 1, in = 'f', out = 'i'; break;
+            case EV_INEG: case EV_IABS: arity = 1, in = out = 'i'; break;
+            case EV_FNEG: case EV_FABS: arity = 1, in = out = 'f'; break;
+            case EV_IADD: case EV_ISUB: case EV_IMUL: case EV_IFLOOR: case EV_IMOD: arity = 2, in = out = 'i'; break;
+            case EV_IDIV: arity = 2, in = 'i', out = 'f'; break;
+            case EV_FADD: case EV_FSUB: case EV_FMUL: case EV_FDIV: arity = 2, in = out = 'f'; break;
+            default: return false;   // EV_X, EV_LOG and unknown opcodes
+        }
+        if (arity == 0) {
+            if (!push || sp == X_DEPTH) return false;
+            st[sp++] = push;
+            continue;
+        }
+        if (sp < arity) return false;
+        for (int i = 0; i < arity; ++i)
+            if (st[sp - 1 - i] != in) return false;
+        sp -= arity;
+        st[sp++] = out;
+    }
+    return sp == 1 && st[0] == want;
+}
+
+// the load slots (as tuple components) and programs of an expression call in kernel-parameter form; f64: the value
+// type op folds
+int expr_view(dampr_ctx *ctx, const dampr_field_expr *x, bool f64, TupleView &tk, ExprView &ev) {
+    ARG_CHECK(ctx, x != nullptr, "null");
+    ARG_CHECK(ctx, x->nloads >= 0 && x->nloads <= DAMPR_EXPR_MAX_LOADS, "0 .. DAMPR_EXPR_MAX_LOADS load slots");
+    tk = TupleView{};
+    ev = ExprView{};
+    tk.n = x->nloads;
+    for (int j = 0; j < x->nloads; ++j) {
+        ARG_CHECK(ctx, x->load_kind[j] >= DAMPR_LOAD_INT && x->load_kind[j] <= DAMPR_LOAD_LEN, "load slot kind");
+        tk.field[j] = x->load_field[j];
+        ev.load_kind[j] = x->load_kind[j];
+    }
+    ARG_CHECK(ctx, x->key_type == DAMPR_EXPR_NONE || x->key_type == DAMPR_EXPR_INT, "key_type");
+    ARG_CHECK(ctx, x->val_type >= DAMPR_EXPR_NONE && x->val_type <= DAMPR_EXPR_F64, "val_type");
+    ARG_CHECK(ctx, x->key_type != DAMPR_EXPR_NONE || x->val_type != DAMPR_EXPR_NONE, "no program");
+    ARG_CHECK(ctx, x->val_type == DAMPR_EXPR_NONE || (x->val_type == DAMPR_EXPR_F64) == f64,
+              "the value program's type must be the one op folds");
+    if (x->key_type != DAMPR_EXPR_NONE) {
+        ARG_CHECK(ctx, expr_program_ok(x->key_prog, x->key_len, 'i', x->load_kind, x->nloads), "malformed key program");
+        ev.key_len = x->key_len;
+        memcpy(ev.key_prog, x->key_prog, sizeof ev.key_prog);
+    }
+    if (x->val_type != DAMPR_EXPR_NONE) {
+        ARG_CHECK(ctx, expr_program_ok(x->val_prog, x->val_len, f64 ? 'f' : 'i', x->load_kind, x->nloads),
+                  "malformed value program");
+        ev.val_len = x->val_len;
+        memcpy(ev.val_prog, x->val_prog, sizeof ev.val_prog);
+    }
+    memcpy(ev.ci, x->ci, sizeof ev.ci);
+    memcpy(ev.cf, x->cf, sizeof ev.cf);
     return DAMPR_OK;
 }
 
@@ -1706,4 +2079,42 @@ extern "C" int32_t dampr_table_fetch_field_keys(dampr_ctx *ctx, dampr_table *t, 
         return DAMPR_ERR_CUDA;
     }
     return DAMPR_OK;
+}
+
+extern "C" int32_t dampr_text_fields_expr(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
+                                          uint64_t own_hi, const dampr_fields_spec *spec, const dampr_field_expr *expr) {
+    if (int r = check_fields_args(ctx, t, tb, own_lo, own_hi, spec)) return r;
+    const bool f64 = spec->op == DAMPR_OP_MIN_F64 || spec->op == DAMPR_OP_MAX_F64;
+    ARG_CHECK(ctx, f64 || spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_MIN_I64 ||
+                       spec->op == DAMPR_OP_MAX_I64,
+              "op must be DAMPR_OP_SUM_I64, DAMPR_OP_MIN_I64, DAMPR_OP_MAX_I64, DAMPR_OP_MIN_F64 or DAMPR_OP_MAX_F64");
+    TupleView tk;
+    ExprView xe;
+    if (int r = expr_view(ctx, expr, f64, tk, xe)) return r;
+    ARG_CHECK(ctx, !f64 || xe.val_len || spec->val_field != DAMPR_FIELD_VAL_ONE, "a float op needs a value");
+    if (own_hi <= own_lo) return DAMPR_OK;
+    const FieldsView tv = fields_view(t, spec, spec->op);
+    wait_uploads(ctx);
+    if (f64) return launch_fold<VK_F64, M_TABLE>(ctx, tb, own_lo, own_hi, spec, tv, RecView{}, &tk, &xe);
+    return launch_fold<VK_INT, M_TABLE>(ctx, tb, own_lo, own_hi, spec, tv, RecView{}, &tk, &xe);
+}
+
+extern "C" int32_t dampr_text_fields_expr_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb,
+                                                  uint64_t own_lo, uint64_t own_hi, const dampr_fields_spec *spec,
+                                                  const dampr_field_expr *expr, dampr_kv *rec) {
+    if (int r = check_fields_args(ctx, t, tb, own_lo, own_hi, spec)) return r;
+    ARG_CHECK(ctx, rec != nullptr, "null");
+    ARG_CHECK(ctx, spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_SUM_F64,
+              "op must be DAMPR_OP_SUM_I64 or DAMPR_OP_SUM_F64");
+    TupleView tk;
+    ExprView xe;
+    if (int r = expr_view(ctx, expr, spec->op == DAMPR_OP_SUM_F64, tk, xe)) return r;
+    ARG_CHECK(ctx, xe.val_len || spec->val_field != DAMPR_FIELD_VAL_ONE, "record mode needs a value");
+    if (own_hi <= own_lo) return DAMPR_OK;
+    const FieldsView tv = fields_view(t, spec, DAMPR_OP_SUM_I64);   // the table counts the lines of each key
+    RecView rv{rec->rec, rec->capacity, nullptr};
+    if (int r = count_records(ctx, t, tb, own_lo, own_hi, tv, rv)) return r;
+    if (spec->op == DAMPR_OP_SUM_F64)
+        return launch_fold<VK_F64, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, tv, rv, &tk, &xe);
+    return launch_fold<VK_INT, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, tv, rv, &tk, &xe);
 }

@@ -606,17 +606,7 @@ int32_t dampr_textbuf_download(dampr_ctx *ctx, dampr_textbuf *tb, uint64_t off, 
 #include <cmath>
 
 namespace {
-enum EvalOp : int32_t {
-    EV_X = 0,      // push the column value (int)
-    EV_CI = 1,     // push int constant ci[arg]
-    EV_CF = 2,     // push float constant cf[arg]
-    EV_I2F = 3,    // float() of the int on top
-    EV_IADD = 4, EV_ISUB = 5, EV_IMUL = 6,
-    EV_FADD = 7, EV_FSUB = 8, EV_FMUL = 9, EV_FDIV = 10,
-    EV_IDIV = 11,  // int / int: true division
-    EV_LOG = 12,   // math.log of the float on top
-    EV_INEG = 13, EV_FNEG = 14,
-};
+// (the opcodes, EvalOp, are common.cuh's: the field scans' programs share them)
 union EvalSlot {
     long long i;
     double f;

@@ -28,6 +28,7 @@ OP_SUM_I64, OP_SUM_F64, OP_COUNT, OP_MIN_I64, OP_MAX_I64, OP_MIN_F64, OP_MAX_F64
 TF_NONASCII, TF_CR, TF_LONGLINE, TF_TABLEFULL, TF_LONGTOKEN, TF_COLLISION = 1, 2, 4, 8, 16, 32
 TF_RECFULL, TF_NEGZERO = 64, 128   # field scans: record buffer full / a float() field parsed to -0.0
 TF_JSON_KEY_KIND, TF_JSON_VAL_KIND = 256, 512   # JSON scans: a key / value member of the other JSON kind
+TF_NAN = 1024   # expression scans: a computed float value is a NaN
 TOK_FLAG_CR_DATA = 0x100
 # delimited-field scans (dampr_text_fields)
 FIELD_KEY_STR, FIELD_KEY_INT = 0, 1
@@ -37,6 +38,10 @@ FIELD_SEP_JSON = 257   # sep of the JSON-lines calls: fields are the members of 
 JSON_MAX_MEMBERS, JSON_MAX_NAME, JSON_MAX_DEPTH = 8, 64, 64
 FIELDS_HALO = 65536
 FIELD_KEYS_MAX = 4   # components of a tuple key (dampr_field_keys)
+# computed keys and values of a field scan (dampr_field_expr): limits, program types, load slot kinds
+EXPR_MAX_OPS, EXPR_MAX_LOADS, EXPR_MAX_DEPTH, EXPR_MAX_CONSTS = 32, 4, 8, 16
+EXPR_NONE, EXPR_INT, EXPR_F64 = 0, 1, 2
+LOAD_INT, LOAD_F64, LOAD_LEN = 0, 1, 2
 # WHERE predicates of a field scan (dampr_field_pred): kinds, comparisons, limits per call
 PRED_STR, PRED_INT, PRED_F64, PRED_NFIELDS, PRED_MEMBER = range(5)
 CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_IN, CMP_NOT_IN = range(8)
@@ -115,6 +120,36 @@ def field_keys(keys):
     for j, (i, kind) in enumerate(keys[:FIELD_KEYS_MAX]):
         k.field[j], k.kind[j] = int(i), int(kind)
     return k
+
+
+class FieldExpr(C.Structure):
+    """dampr_field_expr"""
+    _fields_ = [("key_type", C.c_int32), ("key_len", C.c_int32), ("key_prog", C.c_int32 * EXPR_MAX_OPS),
+                ("val_type", C.c_int32), ("val_len", C.c_int32), ("val_prog", C.c_int32 * EXPR_MAX_OPS),
+                ("ci", C.c_int64 * EXPR_MAX_CONSTS), ("cf", C.c_double * EXPR_MAX_CONSTS), ("nloads", C.c_int32),
+                ("load_field", C.c_int32 * EXPR_MAX_LOADS), ("load_kind", C.c_int32 * EXPR_MAX_LOADS)]
+
+
+def field_expr(expr):
+    """dampr_field_expr of expr = (key program or None, value program or None, int constants, float constants,
+    loads): a program is (EXPR_INT | EXPR_F64, [opcode words]), loads [(field index, LOAD_*)]. Out-of-range lengths
+    are passed on for the library to refuse."""
+    key, val, ci, cf, loads = expr
+    x = FieldExpr()
+    for prog, t, n, words in ((key, "key_type", "key_len", x.key_prog), (val, "val_type", "val_len", x.val_prog)):
+        if prog is not None:
+            setattr(x, t, int(prog[0]))
+            setattr(x, n, len(prog[1]))
+            for i, w in enumerate(prog[1][:EXPR_MAX_OPS]):
+                words[i] = int(w)
+    for i, c in enumerate(ci[:EXPR_MAX_CONSTS]):
+        x.ci[i] = int(c)
+    for i, c in enumerate(cf[:EXPR_MAX_CONSTS]):
+        x.cf[i] = float(c)
+    x.nloads = len(loads)
+    for j, (f, kind) in enumerate(loads[:EXPR_MAX_LOADS]):
+        x.load_field[j], x.load_kind[j] = int(f), int(kind)
+    return x
 
 
 class JsonMembers(C.Structure):
@@ -196,6 +231,8 @@ def load_library():
          vp)
     _sig(lib, "dampr_text_fields_tuple", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), C.POINTER(FieldKeys))
     _sig(lib, "dampr_text_fields_tuple_records", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), C.POINTER(FieldKeys), vp)
+    _sig(lib, "dampr_text_fields_expr", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), C.POINTER(FieldExpr))
+    _sig(lib, "dampr_text_fields_expr_records", vp, vp, vp, u64, u64, C.POINTER(FieldsSpec), C.POINTER(FieldExpr), vp)
     _sig(lib, "dampr_table_fetch_field_keys", vp, vp, vp, i32, C.POINTER(FieldKeys), C.POINTER(u32), C.POINTER(vp),
          vp, vp, u64, pu64)
     _sig(lib, "dampr_table_stats", vp, vp, pu64)
@@ -660,6 +697,20 @@ class Table(object):
         s, k = fields_spec(spec, cr_is_data, preds), field_keys(keys)
         self.ctx.check(self.ctx.lib.dampr_text_fields_tuple_records(self.ctx.h, self.h, tb.h, int(lo), int(hi),
                                                                     C.byref(s), C.byref(k), kv.h))
+
+    def fields_expr(self, tb, lo, hi, spec, expr, cr_is_data=False, preds=()):
+        """fields() with a computed key and / or value: expr as field_expr() (lowering.text_fields_expr's programs);
+        a key program's int keys are coded as FIELD_KEY_INT keys (fetch() decodes them), spec's key or value is read
+        where expr has no program"""
+        s, x = fields_spec(spec, cr_is_data, preds), field_expr(expr)
+        self.ctx.check(self.ctx.lib.dampr_text_fields_expr(self.ctx.h, self.h, tb.h, int(lo), int(hi), C.byref(s),
+                                                           C.byref(x)))
+
+    def fields_expr_records(self, tb, lo, hi, spec, expr, kv, cr_is_data=False, preds=()):
+        """fields_records() with a computed key and / or value, expr as fields_expr()"""
+        s, x = fields_spec(spec, cr_is_data, preds), field_expr(expr)
+        self.ctx.check(self.ctx.lib.dampr_text_fields_expr_records(self.ctx.h, self.h, tb.h, int(lo), int(hi),
+                                                                   C.byref(s), C.byref(x), kv.h))
 
     def fetch_field_keys(self, tb, sep, keys):
         """(columns, counts, codes) of a tuple-key table, decoded on the device from each entry's representative line:

@@ -731,9 +731,11 @@ def depends_on(e, argi, fields=None):
 
 
 # ---- numeric expressions evaluated natively (dampr_host_eval_f64) -------------------------------------------------
+# the opcodes of csrc/common.cuh's EvalOp
 _EV = dict(X=0, CI=1, CF=2, I2F=3, IADD=4, ISUB=5, IMUL=6, FADD=7, FSUB=8, FMUL=9, FDIV=10, IDIV=11, LOG=12,
-           INEG=13, FNEG=14)
+           INEG=13, FNEG=14, LOAD=15, NF=16, IFLOOR=17, IMOD=18, IABS=19, FABS=20, F2I=21)
 _EV_BIN = {"+": ("IADD", "FADD"), "-": ("ISUB", "FSUB"), "*": ("IMUL", "FMUL")}
+EXPR_MAX_OPS, EXPR_MAX_LOADS, EXPR_MAX_DEPTH, EXPR_MAX_CONSTS = 32, 4, 8, 16   # include/dampr_b200.h
 
 
 def _callee(f):
@@ -745,12 +747,18 @@ def _callee(f):
     return None
 
 
-def numeric_program(e, field, scalar, argi=1):
+def numeric_program(e, field, scalar, argi=1, result="f", leaf=None):
     """Postfix program of dampr_host_eval_f64 for a float-valued expression over one int64 field `field` of argument
     `argi` (the column), the other argument as the broadcast value `scalar` (an int or a float) and int / float
     constants, built from + - * /, unary -, float() and math.log — typed as CPython types it (int operands of a float
     operation are converted first, int / int is true division). Returns (program, int constants, float constants),
-    or None for anything outside that set (the caller then calls the function in Python)."""
+    or None for anything outside that set (the caller then calls the function in Python).
+
+    With `leaf` (a field scan's program, dampr_field_expr) the arguments are not read as a column or a scalar: leaf(x)
+    gives (opcode word, "i" | "f") for a node that is a load or a field count, else None. Such a program may also use
+    // and % of ints, abs() and int() of a float, not math.log; it is an int program under result "i", and it stays
+    within the device's limits (EXPR_MAX_OPS operations, EXPR_MAX_DEPTH stack values, EXPR_MAX_CONSTS constants of
+    each type)."""
     import math
     prog, ci, cf = [], [], []
 
@@ -775,6 +783,13 @@ def numeric_program(e, field, scalar, argi=1):
     def walk(x):
         if not isinstance(x, E):
             return None
+        if leaf is not None:
+            got = leaf(x)
+            if got is not None:
+                prog.append(got[0])
+                return got[1]
+            if x.op in ("sub", "arg"):
+                return None
         if x.op == "sub" and _is_arg(x.a, argi):
             ok, i = _const(x.b)
             if ok and type(i) is int and i == field:
@@ -790,6 +805,11 @@ def numeric_program(e, field, scalar, argi=1):
             if t:
                 prog.append(_EV["INEG" if t == "i" else "FNEG"])
             return t
+        if leaf is not None and x.op == "bin" and x.a in ("//", "%"):   # float // and % are not lowered
+            if walk(x.b) != "i" or walk(x.c) != "i":
+                return None
+            prog.append(_EV["IFLOOR" if x.a == "//" else "IMOD"])
+            return "i"
         if x.op == "bin" and x.a in ("+", "-", "*", "/"):
             tl = walk(x.b)
             if not tl:
@@ -813,7 +833,17 @@ def numeric_program(e, field, scalar, argi=1):
             f = _callee(x.a)
             if f is float:
                 return to_float(walk(x.b[0]))
-            if f is math.log:
+            if leaf is not None and f is abs:
+                t = walk(x.b[0])
+                if t:
+                    prog.append(_EV["IABS" if t == "i" else "FABS"])
+                return t
+            if leaf is not None and f is int:
+                t = walk(x.b[0])
+                if t == "f":
+                    prog.append(_EV["F2I"])
+                return "i" if t else None
+            if leaf is None and f is math.log:
                 t = to_float(walk(x.b[0]))
                 if t:
                     prog.append(_EV["LOG"])
@@ -821,6 +851,182 @@ def numeric_program(e, field, scalar, argi=1):
         return None
 
     t = walk(e)
-    if t != "f" or len(prog) > 256:
+    if t != result or len(prog) > (256 if leaf is None else EXPR_MAX_OPS):
         return None
+    if leaf is not None:
+        depth = top = 0
+        for w in prog:
+            op = w & 0xFF
+            depth += 1 if op in (_EV["CI"], _EV["CF"], _EV["LOAD"], _EV["NF"]) else 0 if op in _EV_UNARY else -1
+            top = max(top, depth)
+        if top > EXPR_MAX_DEPTH or len(ci) > EXPR_MAX_CONSTS or len(cf) > EXPR_MAX_CONSTS:
+            return None
     return prog, ci, cf
+
+
+_EV_UNARY = {_EV[k] for k in ("I2F", "LOG", "INEG", "FNEG", "IABS", "FABS", "F2I")}
+
+
+# ---- computed keys and values of a field fold (dampr_text_fields_expr) --------------------------------------------
+EV_CI = _EV["CI"]
+FIELD_EXPR = "expr"   # value_index of a text_fields_expr spec whose value is computed by its program
+LOAD_INT, LOAD_F64, LOAD_LEN = 0, 1, 2   # load slot kinds (DAMPR_LOAD_*)
+
+
+class _NoCompose(Exception):
+    pass
+
+
+def _compose(e, m, used):
+    """e, a tree over argument 0, with the argument replaced by m, the tree of the map in front (x[i] of a tuple m is
+    its element i, whose index goes into `used`; the whole m counts as element -1)"""
+    if not isinstance(e, E):
+        return e
+    op = e.op
+    if op == "arg":
+        if e.a != 0:
+            raise _NoCompose()
+        used.add(-1)
+        return m
+    if op == "sub" and _is_arg(e.a) and isinstance(m, E) and m.op == "tuple":
+        ok, i = _const(e.b)
+        if not ok or type(i) is not int or not -len(m.a) <= i < len(m.a):
+            raise _NoCompose()
+        used.add(i % len(m.a))
+        return m.a[i]
+    if op in ("const", "obj"):
+        return e
+    if op == "call":
+        return E(op, _compose(e.a, m, used), tuple(_compose(x, m, used) for x in e.b))
+    if op == "tuple":
+        return E(op, tuple(_compose(x, m, used) for x in e.a))
+    if op == "attr":
+        return E(op, _compose(e.a, m, used), e.b)
+    if op in ("bin", "cmp"):
+        return E(op, e.a, _compose(e.b, m, used), _compose(e.c, m, used))
+    if op == "neg":
+        return E(op, _compose(e.a, m, used))
+    if op == "sub":
+        return E(op, _compose(e.a, m, used), _compose(e.b, m, used))
+    raise _NoCompose()
+
+
+def split_of(fn):
+    """the separator of a one-argument `lambda l: l.split(S)` / `l.split()` (SEP_WS), else None"""
+    if not (isinstance(fn, types.FunctionType) and fn.__code__.co_argcount == 1):
+        return None
+    return _split_sep(analyze(fn), True)
+
+
+def text_fields_expr(key_fn, value_fn, map_fn=None):
+    """Device field-scan spec of a keyed(key_fn, value_fn) over text lines, behind an optional map(map_fn), for the
+    shapes text_fields_spec refuses: a key that is an int expression (a constant one included, e.g. mean()'s default
+    `lambda x: 1`) and / or a value that is an int or float expression, over the leaves int(R[j]), float(R[j]),
+    len(R), len(R[j]) and int / float constants, with + - * / // % (// and % of ints), unary -, abs(), float() and
+    int() — typed as CPython types them. R is l.split(S) or l.split() of the line.
+
+    map_fn may be l.split(S) / l.split(), or return an expression over the line or a tuple of such; the key and value
+    functions are composed with its tree ((...)[i] of its tuple resolves to element i). Every element of such a map
+    must be used by the key or the value: the device evaluates only what they read, and an unused element could
+    raise in Python.
+
+    Returns (sep, key_index, key_kind, value_index, value_kind, mean, expr) with sep the split's separator (SEP_WS
+    for split(); None when no field is read), key_kind FIELD_STR / FIELD_INT (a projection, key_index its field) or
+    FIELD_INT with key_index None (a key program), value_index the field of an int() / float() value, None for the
+    constant 1 or FIELD_EXPR for a value program, value_kind FIELD_INT / FIELD_FLOAT, mean as text_fields_spec, and
+    expr = (key program or None, value program or None, int constants, float constants, loads) with a program
+    ("i" | "f", [opcode words]) and loads [(field index, LOAD_*)]. expr is None when the composition left bare
+    projections only (the plain scan's spec). None for any other shape."""
+    fns = [f for f in (key_fn, value_fn, map_fn) if f is not None]
+    if not all(isinstance(f, types.FunctionType) and f.__code__.co_argcount == 1 for f in fns):
+        return None
+    ke, ve = analyze(key_fn), analyze(value_fn)
+    if ke is None or ve is None:
+        return None
+    mean = ve.op == "tuple" and len(ve.a) == 2
+    if mean:
+        inner = _inline_call_of_arg(ve.a[0])
+        if inner is None or not _is_one(ve.a[1]):
+            return None
+        ve = inner
+    if map_fn is not None:
+        me = analyze(map_fn)
+        if me is None:
+            return None
+        used = set()
+        try:
+            ke, ve = _compose(ke, me, used), _compose(ve, me, used)
+        except _NoCompose:
+            return None
+        if _split_sep(me, True) is None:
+            need = set(range(len(me.a))) if me.op == "tuple" else {-1}
+            if not need <= used and not (me.op == "tuple" and -1 in used):
+                return None
+
+    seps, loads = set(), []
+
+    def record(x):
+        sep = _split_sep(x, True)
+        if sep is not None:
+            seps.add(sep)
+        return sep
+
+    def slot(i, kind):
+        if (i, kind) not in loads:
+            loads.append((i, kind))
+        return _EV["LOAD"] | loads.index((i, kind)) << 8
+
+    def leaf(x):
+        if not (isinstance(x, E) and x.op == "call" and isinstance(x.b, tuple) and len(x.b) == 1):
+            return None
+        f = _callee(x.a)
+        if f is len:
+            if record(x.b[0]) is not None:
+                return _EV["NF"], "i"
+            p = _field_proj(x.b[0], record)
+            return (slot(p[1], LOAD_LEN), "i") if p is not None and p[0] == FIELD_STR else None
+        if f in (int, float):
+            p = _value_proj(x, record)
+            if p is not None:
+                return (slot(p[1], LOAD_INT), "i") if p[0] == FIELD_INT else (slot(p[1], LOAD_F64), "f")
+        return None
+
+    k = _field_proj(ke, record)
+    kprog = None
+    if k is None:
+        kprog = numeric_program(ke, None, None, result="i", leaf=leaf)
+        if kprog is None:
+            return None
+    vprog, v, vtype = None, None, "i"
+    if not (_is_one(ve) and not mean):
+        v = _value_proj(ve, record)
+        if v is None:
+            vprog = numeric_program(ve, None, None, result="i", leaf=leaf)
+            if vprog is None:
+                vprog, vtype = numeric_program(ve, None, None, result="f", leaf=leaf), "f"
+            if vprog is None:
+                return None
+    if len(seps) > 1 or len(loads) > EXPR_MAX_LOADS:
+        return None
+    sep = seps.pop() if seps else None
+    if kprog is None and vprog is None:   # bare projections after the composition: the plain scan's spec
+        return (sep, k[1], k[0], None if v is None else v[1], FIELD_INT if v is None else v[0], mean, None)
+    progs, ci, cf = [], [], []
+    for p in (kprog, vprog):   # one pool of constants: the value program's indices move past the key program's
+        if p is None:
+            progs.append(None)
+            continue
+        words, pci, pcf = p
+        out = []
+        for w in words:
+            op = w & 0xFF
+            out.append(op | (w >> 8) + len(ci) << 8 if op == _EV["CI"] else
+                       op | (w >> 8) + len(cf) << 8 if op == _EV["CF"] else w)
+        progs.append(("i" if p is kprog else vtype, out))
+        ci, cf = ci + pci, cf + pcf
+    if len(ci) > EXPR_MAX_CONSTS or len(cf) > EXPR_MAX_CONSTS:
+        return None
+    vkind = (FIELD_INT if v is None else v[0]) if vprog is None else \
+        (FIELD_FLOAT if progs[1][0] == "f" else FIELD_INT)
+    return (sep, None if kprog else k[1], FIELD_INT if kprog else k[0],
+            FIELD_EXPR if vprog else None if v is None else v[1], vkind, mean, (progs[0], progs[1], ci, cf, loads))

@@ -748,8 +748,9 @@ class FieldScan(TextScan):
     HALO = dev.FIELDS_HALO   # a line longer than the kernel's window is measured up to 64 KB past its start
     REC_BYTES = 32           # per record: the record and the sort's scratch copy
 
-    def __init__(self, runner, sources, spec, op, stage, mean, preds=()):
+    def __init__(self, runner, sources, spec, op, stage, mean, preds=(), expr=None):
         TextScan.__init__(self, runner, sources, None)
+        self.expr = expr     # computed key / value programs (device.field_expr) for dampr_text_fields_expr, or None
         self.spec = spec     # (separator byte or FIELD_SEP_WS, key index, key kind, value index or FIELD_VAL_ONE)
         # a tuple key (key kind KEY_TUPLE): its components go to the tuple calls, the spec's key field is not read
         self.key_comps = spec[1] if spec[2] == KEY_TUPLE else None
@@ -774,7 +775,9 @@ class FieldScan(TextScan):
             spec = (spec[0], 0, dev.FIELD_KEY_STR) + spec[3:]
         if not self.records:
             # a stage without filters makes exactly the plain call
-            if self.key_comps is not None:
+            if self.expr is not None:
+                tab.fields_expr(tb, lo, hi, spec, self.expr, cr, **self._where)
+            elif self.key_comps is not None:
                 tab.fields_tuple(tb, lo, hi, spec, self.key_comps, cr, **self._where)
             else:
                 tab.fields(tb, lo, hi, spec, cr, **self._where)
@@ -783,7 +786,9 @@ class FieldScan(TextScan):
             # a first guess of one record per 32 bytes of text; a scan with more lines is repeated once with a
             # buffer of the exact size (DAMPR_TF_RECFULL)
             self._records_buffer(min(tb.n // 32 + 4096, self._free_bytes() // (2 * self.REC_BYTES)))
-        if self.key_comps is not None:
+        if self.expr is not None:
+            tab.fields_expr_records(tb, lo, hi, spec, self.expr, self._rec, cr, **self._where)
+        elif self.key_comps is not None:
             tab.fields_tuple_records(tb, lo, hi, spec, self.key_comps, self._rec, cr, **self._where)
         else:
             tab.fields_records(tb, lo, hi, spec, self._rec, cr, **self._where)
@@ -828,6 +833,8 @@ class FieldScan(TextScan):
             raise NotLowerable("64-bit key-code collision between two long keys")
         if self.float_values and flags & dev.TF_NEGZERO:
             raise NotLowerable("-0.0 among the float() values: Python's result depends on the order of the arguments")
+        if self.float_values and self.op != dev.OP_SUM_F64 and flags & dev.TF_NAN:
+            raise NotLowerable("a computed NaN under min/max: Python's result depends on the order of the arguments")
         if self.records and flags & dev.TF_RECFULL:
             if self._rec_regrown:
                 raise NotLowerable("field records overflow their buffer")
@@ -1125,7 +1132,9 @@ def _match_text_fields(stage, inputs):
     (+, +), over text, each filter one lowering.field_predicate on the key's separator: (sources, (sep byte or
     FIELD_SEP_WS, key index, key kind, value index or FIELD_VAL_ONE), op, mean, device predicates) or None. A tuple
     key of field projections has key kind KEY_TUPLE and, as its key index, the components ((index, FIELD_KEY_STR |
-    FIELD_KEY_INT), ...)."""
+    FIELD_KEY_INT), ...). A sixth element is the stage's computed key / value programs (lowering.text_fields_expr, in
+    device.field_expr form) for the shapes text_fields_spec refuses, else None: the map may then also compute an
+    expression or a tuple of them (no filter may follow such a map), a key program's keys are FIELD_KEY_INT keys."""
     if not isinstance(stage, GMap) or len(inputs) != 1:
         return None
     src = _text_files(inputs[0])
@@ -1140,10 +1149,19 @@ def _match_text_fields(stage, inputs):
         return None
     keyed = ks[-1][1]
     at = kinds.index("map") if "map" in kinds else None
-    spec = lowering.text_fields_spec(keyed.fn, keyed.fn2, ks[at][1].fn if at is not None else None, whitespace=True,
-                                     tuple_keys=True)
+    mapfn = ks[at][1].fn if at is not None else None
+    spec = lowering.text_fields_spec(keyed.fn, keyed.fn2, mapfn, whitespace=True, tuple_keys=True)
+    expr = None
     if spec is None:
-        return None
+        spec = lowering.text_fields_expr(keyed.fn, keyed.fn2, mapfn)
+        if spec is None:
+            return None
+        msep = lowering.split_of(mapfn) if at is not None else None
+        if at is not None and msep is None and "filter" in kinds[at + 1:]:
+            return None   # a filter over the computed record of the map: not a field predicate
+        spec, expr = spec[:6], spec[6]
+        if spec[0] is None and msep is not None:
+            spec = (msep,) + spec[1:]
     sep, ki, kkind, vi, vkind, mean = spec
     if kkind == lowering.FIELD_TUPLE:
         ki = tuple((i, dev.FIELD_KEY_INT if k == lowering.FIELD_INT else dev.FIELD_KEY_STR) for i, k in ki)
@@ -1151,6 +1169,8 @@ def _match_text_fields(stage, inputs):
     for i, (k, o) in enumerate(ks[:-1]):
         if k == "filter":
             p = lowering.field_predicate(o.fn, sep if at is not None and i > at else None, whitespace=True)
+            if p is not None and sep is None:   # a computed key and value that read no field: the filters' split
+                sep = p[0]
             if p is None or p[0] != sep:
                 return None
             preds.append(_device_pred(p))
@@ -1167,10 +1187,18 @@ def _match_text_fields(stage, inputs):
         if kind not in (lowering.ADD, lowering.MIN, lowering.MAX):
             return None
         op = (_FOLD_OPS_F64 if vkind == lowering.FIELD_FLOAT else _FOLD_OPS)[kind]
+    if expr is not None:
+        kp, vp, ci, cf, loads = expr
+        types = {"i": dev.EXPR_INT, "f": dev.EXPR_F64}
+        expr = (None if kp is None else (types[kp[0]], tuple(kp[1])), None if vp is None else (types[vp[0]], tuple(vp[1])),
+                tuple(ci), tuple(cf), tuple(loads))
+        ki = 0 if ki is None else ki      # (the programs replace the spec's key and value fields)
+        vi = 0 if vi == lowering.FIELD_EXPR else vi
+        sep = "," if sep is None else sep   # nothing is split: any separator
     return src, (dev.FIELD_SEP_WS if sep == lowering.SEP_WS else ord(sep), ki,
                  KEY_TUPLE if kkind == lowering.FIELD_TUPLE else
                  dev.FIELD_KEY_INT if kkind == lowering.FIELD_INT else dev.FIELD_KEY_STR,
-                 dev.FIELD_VAL_ONE if vi is None else vi), op, mean, tuple(preds)
+                 dev.FIELD_VAL_ONE if vi is None else vi), op, mean, tuple(preds), expr
 
 
 def _match_json_fields(stage, inputs):
@@ -1320,10 +1348,11 @@ def _lower_map(runner, stage, inputs, si):
     if m is not None:
         if dist.active():
             raise NotLowerable("the field scan runs on one process")
-        src, spec, op, mean, preds = m
-        scan = FieldScan(runner, src, spec, op, stage, mean, preds).run()
+        src, spec, op, mean, preds, expr = m
+        scan = FieldScan(runner, src, spec, op, stage, mean, preds, expr).run()
         opname = ("mean_f64" if op == dev.OP_SUM_F64 else "mean_i64") if mean else \
-            "count" if spec[3] == dev.FIELD_VAL_ONE and op == dev.OP_SUM_I64 else _FIELD_OP_NAMES[op]
+            "count" if spec[3] == dev.FIELD_VAL_ONE and op == dev.OP_SUM_I64 and (expr is None or expr[1] is None) \
+            else _FIELD_OP_NAMES[op]
         detail = "op=%s bytes=%d lines=%d groups=%d host_lines=%d" % (opname, scan.nbytes, scan.n_lines, scan.groups,
                                                                       scan.host_lines)
         if preds:
@@ -1332,6 +1361,10 @@ def _lower_map(runner, stage, inputs, si):
             detail += " sep=ws"
         if spec[2] == KEY_TUPLE:
             detail += " key=tuple%d" % len(spec[1])
+        if expr is not None and expr[1] is not None:
+            detail += " value=expr"
+        if expr is not None and expr[0] is not None:
+            detail += " key=const" if len(expr[0][1]) == 1 and expr[0][1][0] & 0xFF == lowering.EV_CI else " key=expr"
         runner.stats.add(stage, "device text fields scan+combine", detail)
         return Frame(scan.keys, [scan.values], scalar=True, combined=True)
     m = _match_json_fields(stage, inputs)

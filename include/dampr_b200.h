@@ -299,6 +299,56 @@ int32_t dampr_text_fields_tuple(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *t
 int32_t dampr_text_fields_tuple_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
                                         uint64_t own_hi, const dampr_fields_spec *spec, const dampr_field_keys *keys,
                                         dampr_kv *rec);
+/* ---- computed keys and values: `int(r[2]) * int(r[3])`, `float(r[5]) / 1000`, `int(r[0]) // 3600`, `len(r)`,
+ *      `len(r[1])`, constant keys (`lambda x: 1`) ------------------------------------------------------------------
+ * The same folds, predicates, line rules and stats as dampr_text_fields / dampr_text_fields_records (sep a separator
+ * byte or DAMPR_FIELD_SEP_WS), with the key and / or the value computed per line by a postfix program over the typed
+ * stack of csrc/common.cuh's EvalOp opcodes (op | arg << 8; every opcode but EV_X and EV_LOG). Its leaves are int
+ * and float constants (ci[arg], cf[arg]), the line's field count (EV_NF) and load slots (EV_LOAD arg): slot j is
+ * int(), float() or len() of field load_field[j] of the line's split, the field rules of the scan above (a missing
+ * field, or an int() / float() field the device does not parse, makes the line a fallback line). The key program
+ * (key_type DAMPR_EXPR_INT) replaces spec->key_field / key_kind: the key is its int64 v, coded v ^ 2^63 as an int
+ * key. The value program (val_type DAMPR_EXPR_INT or DAMPR_EXPR_F64, the type op folds) replaces spec->val_field.
+ * DAMPR_EXPR_NONE keeps the spec's key or value.
+ * - A line is taken only when every operation reaches CPython's result: a zero divisor of / // % (int or float),
+ *   INT64_MIN // -1, an int + - * unary - or abs() leaving int64, int / int with an operand beyond +-2^53, int() of a
+ *   NaN, an infinity or a float outside int64, and a key equal to INT64_MIN make it a fallback line. Float operations
+ *   are single IEEE roundings (no contraction), int -> float rounds half-even, // and % floor towards -inf.
+ * - A computed float value that is -0.0 sets DAMPR_TF_NEGZERO, a NaN sets DAMPR_TF_NAN (both matter under min / max).
+ * - With a key program each CTA folds its lines' values of up to 32 key codes in shared memory and inserts each code
+ *   once (a constant key or a few buckets would otherwise send every line to one table slot).
+ * Malformed programs return DAMPR_ERR_ARG: a stack underflow, a depth above DAMPR_EXPR_MAX_DEPTH, a final depth other
+ * than 1, an unknown opcode, an operand of the wrong type, a constant or load slot out of range, a result type that
+ * does not match op, more than DAMPR_EXPR_MAX_OPS operations, or no program at all. */
+#define DAMPR_EXPR_MAX_OPS 32
+#define DAMPR_EXPR_MAX_LOADS 4
+#define DAMPR_EXPR_MAX_DEPTH 8
+#define DAMPR_EXPR_MAX_CONSTS 16
+#define DAMPR_EXPR_NONE 0
+#define DAMPR_EXPR_INT 1
+#define DAMPR_EXPR_F64 2
+#define DAMPR_LOAD_INT 0    /* int(line.split(sep)[field]): [+-]?[0-9]{1,18}                                      */
+#define DAMPR_LOAD_F64 1    /* float(line.split(sep)[field]): the float() rule above                               */
+#define DAMPR_LOAD_LEN 2    /* len(line.split(sep)[field]), an int                                                 */
+#define DAMPR_TF_NAN 1024u  /* an expression scan computed a NaN value                                             */
+typedef struct dampr_field_expr {
+    int32_t key_type;                          /* DAMPR_EXPR_NONE | DAMPR_EXPR_INT                                */
+    int32_t key_len;                           /* operations of the key program                                  */
+    int32_t key_prog[DAMPR_EXPR_MAX_OPS];
+    int32_t val_type;                          /* DAMPR_EXPR_NONE | DAMPR_EXPR_INT | DAMPR_EXPR_F64              */
+    int32_t val_len;
+    int32_t val_prog[DAMPR_EXPR_MAX_OPS];
+    int64_t ci[DAMPR_EXPR_MAX_CONSTS];         /* int constants, shared by both programs                         */
+    double cf[DAMPR_EXPR_MAX_CONSTS];          /* float constants                                                */
+    int32_t nloads;                            /* 0 .. DAMPR_EXPR_MAX_LOADS                                      */
+    int32_t load_field[DAMPR_EXPR_MAX_LOADS];  /* i of line.split(sep)[i]; negative counts from the end          */
+    int32_t load_kind[DAMPR_EXPR_MAX_LOADS];   /* DAMPR_LOAD_*                                                   */
+} dampr_field_expr;
+int32_t dampr_text_fields_expr(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo, uint64_t own_hi,
+                               const dampr_fields_spec *spec, const dampr_field_expr *expr);
+int32_t dampr_text_fields_expr_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,
+                                       uint64_t own_hi, const dampr_fields_spec *spec, const dampr_field_expr *expr,
+                                       dampr_kv *rec);
 /* decode a tuple-key table ON THE DEVICE: each entry's representative line is split again (sep and keys as in the
  * scan) into one column per component. Two phases: cols == NULL sets *n (entries) and widths[j] (the longest STR
  * component j, 0 for INT components) only. Then cols[j] = uint8[*n * widths[j]] (STR: NUL-padded, widths[j] >= 1,

@@ -7,7 +7,8 @@ page-cache-warm file, the host-map MB/s on a sample, and whether the device and 
 
     python tools/fields_bench.py [--gb 2] [--keys 1000000] [--reps 3] [--sample-mb 32] [--out DIR]
                                  [--value int|float] [--op sum|min|max|mean] [--where none|str|int|float|set]
-                                 [--sep comma|ws] [--key-fields 1|2|3]
+                                 [--sep comma|ws] [--key-fields 1|2|3] [--expr none|product|ratio|nfields]
+                                 [--key field|const|bucket]
 
 --value float writes the value field as float text (even lines "%.6f", odd lines repr() of the double, right-aligned
 in a 24-byte field) and folds float(r[2]); --op picks `+` (fold_by), min / max (a_group_by().reduce) or mean(). A run
@@ -33,6 +34,16 @@ key has about twice as many groups as the single key (under --sep ws the filler'
 runs around it, which multiplies the groups; "distinct_keys" says how many). It works with every other option of the CSV rows, and the JSON
 line also holds "key_fields" and "fetch_to_frame_ms" (the time from the table fetch to the key column of Python
 tuples, best run).
+
+--expr and --key fold computed values and keys (the expression builds of the field kernel). product and ratio carve a
+quantity field of 1-999 ("%03d") out of the filler, behind the value, so every line keeps its LINE bytes and
+r[2] is the value, r[3] the quantity:
+  product  int(r[2]) * int(r[3])
+  ratio    int(r[2]) / int(r[3])      (a float value)
+  nfields  map(lambda l: len(l.split())) in front of the keyed functions, the README's stage; --key const only
+--key const groups everything under `lambda r: 1`, bucket under int(r[2]) // 1000 (about 200 keys), field under r[0]
+(the default). They take --sep comma and ws (nfields: ws only), --op, and --value int; the JSON line then also holds
+"expr" and "key", and whether the host-map sample agrees (float values: within the sum bound above).
 
 --format json writes JSON lines of JLINE bytes instead: {"user": "u%07d", "n": int, "status": an int or a string,
 "latency": float, "meta": {"user": "decoy", ...}, "pad": filler}, padded with JSON whitespace after the numbers, and
@@ -184,6 +195,67 @@ def rewrite_filler(text, seed, key_fields):
 
 
 KEY_FNS = {1: lambda r: r[0], 2: lambda r: (r[0], r[1]), 3: lambda r: (r[0], r[1], r[-3])}
+EXPR_KEYS = {"field": lambda r: r[0], "const": lambda r: 1, "bucket": lambda r: int(r[2]) // 1000}
+EXPR_VALUES = {"none": lambda r: int(r[2]), "product": lambda r: int(r[2]) * int(r[3]),
+               "ratio": lambda r: int(r[2]) / int(r[3])}
+
+
+def carve_quantity(text, seed, ws):
+    """--expr product / ratio: the rows of csv_text with the filler 4 bytes shorter and a quantity field of 1-999
+    behind the value: key ',' filler ',' value ',' qty '\\n', LINE bytes each (ws: a blank before the quantity,
+    which whitespace_rows keeps)"""
+    rows = text.reshape(-1, LINE)
+    rng = np.random.default_rng(seed)
+    step = 1 << 20
+    for a in range(0, len(rows), step):
+        t = rows[a:a + step]
+        t[:, 89:95] = t[:, 93:99].copy()
+        t[:, 88] = ord(",")
+        t[:, 95] = ord(" " if ws else ",")
+        q = rng.integers(1, 1000, size=len(t))
+        for p in range(3):
+            t[:, 98 - p] = 48 + (q // 10 ** p) % 10
+    return text
+
+
+def expr_job(Dampr, src, expr, key, op, sep):
+    """the --expr / --key stage"""
+    d = Dampr.read_input(src)
+    if expr == "nfields":
+        d = d.map(lambda v: len(v.split()))
+        kf, vf = (lambda x: 1), (lambda x: x)
+    else:
+        d = d.map(splitter(sep))
+        kf, vf = EXPR_KEYS[key], EXPR_VALUES[expr]
+    if op == "mean":
+        return d.mean(kf, vf)
+    if op in ("min", "max"):
+        return d.a_group_by(kf, vf).reduce(min if op == "min" else max)
+    return d.fold_by(kf, value=vf, binop=lambda a, b: a + b)
+
+
+def expr_fold(sample, expr, key, op, sep):
+    """the --expr / --key stage as plain Python over the sample's lines: ({key: result}, {key: (lines, sum |v|)})"""
+    out, mag = {}, {}
+    lines = sample.decode("ascii").split("\n")[:-1]
+    if expr == "nfields":
+        rows = ((1, len(l.split())) for l in lines)
+    else:
+        kf, vf = EXPR_KEYS[key], EXPR_VALUES[expr]
+        rows = ((kf(r), vf(r)) for r in map(splitter(sep), lines))
+    for k, v in rows:
+        n, m = mag.get(k, (0, 0.0))
+        mag[k] = (n + 1, m + abs(v))
+        if op == "mean":
+            s, c = out.get(k, (0, 0))
+            out[k] = (s + v, c + 1)
+        elif k in out:
+            out[k] = out[k] + v if op == "sum" else (min if op == "min" else max)(out[k], v)
+        else:
+            out[k] = v
+    if op == "mean":
+        out = {k: s / float(c) for k, (s, c) in out.items()}
+    return out, mag
 
 
 def splitter(sep):
@@ -296,7 +368,14 @@ def main():
     ap.add_argument("--sep", choices=("comma", "ws", ","), default="comma")
     ap.add_argument("--format", choices=("csv", "json"), default="csv")
     ap.add_argument("--key-fields", type=int, choices=(1, 2, 3), default=1)
+    ap.add_argument("--expr", choices=("none", "product", "ratio", "nfields"), default="none")
+    ap.add_argument("--key", choices=("field", "const", "bucket"), default="field")
     a = ap.parse_args()
+    computed = a.expr != "none" or a.key != "field"
+    if computed and (a.format != "csv" or a.value != "int" or a.where != "none" or a.key_fields != 1):
+        ap.error("--expr and --key take neither --format json, --value float, --where nor --key-fields")
+    if a.expr == "nfields" and (a.sep != "ws" or a.key != "const"):
+        ap.error("--expr nfields is the README's stage: --sep ws --key const")
     if a.sep == ",":
         a.sep = "comma"
     if a.format == "json":
@@ -305,7 +384,7 @@ def main():
         a.sep = "json"
     if a.where == "int" and a.value != "int":
         ap.error("--where int needs --value int (int() of a float field raises)")
-    default = a.value == "int" and a.op == "sum" and a.key_fields == 1
+    default = a.value == "int" and a.op == "sum" and a.key_fields == 1 and not computed
     K = a.key_fields
 
     from dampr_b200 import Dampr, device as dev, plan
@@ -319,8 +398,10 @@ def main():
     else:
         text = csv_text(2026, n_lines, a.keys) if a.value == "int" else float_text(2026, n_lines, a.keys)
         text = rewrite_filler(text, 2028, K)
+        if a.expr in ("product", "ratio"):
+            text = carve_quantity(text, 2029, a.sep == "ws")
     if a.sep == "ws":
-        text = whitespace_rows(text, 2027, 6 if a.value == "int" else FVAL)
+        text = whitespace_rows(text, 2027, 10 if a.expr in ("product", "ratio") else 6 if a.value == "int" else FVAL)
     nbytes = len(text)
     pin = dev.PinnedBuffer(nbytes)
     pin.array[:] = text
@@ -343,7 +424,9 @@ def main():
     def timed(src, where="none"):
         ctx.timings_reset()
         t0 = time.perf_counter()
-        n = len(list(job(Dampr, src, a.value, a.op, where, a.sep, K).run()))
+        stage = expr_job(Dampr, src, a.expr, a.key, a.op, a.sep) if computed else \
+            job(Dampr, src, a.value, a.op, where, a.sep, K)
+        n = len(list(stage.run()))
         dt = time.perf_counter() - t0
         stages = runner_mod.LAST_STATS.stages
         assert "device text fields scan+combine" in stages[0][1], stages
@@ -372,7 +455,9 @@ def main():
     sample_lines = max(1, int(a.sample_mb * 1e6) // line)
     sample = pin.array[:sample_lines * line].tobytes()
     t0 = time.perf_counter()
-    if default and a.sep != "json":
+    if computed:
+        host, host_mag = expr_fold(sample, a.expr, a.key, a.op, a.sep)
+    elif default and a.sep != "json":
         host = {}
         split = splitter(a.sep)
         for l in sample.decode("ascii").split("\n")[:-1]:
@@ -384,7 +469,8 @@ def main():
     host_s = time.perf_counter() - t0
     spin = dev.PinnedBuffer(len(sample))
     spin.array[:] = np.frombuffer(sample, dtype=np.uint8)
-    got = dict(job(Dampr, plan.MemoryText(spin.array), a.value, a.op, sep=a.sep, key_fields=K).run())
+    got = dict((expr_job(Dampr, plan.MemoryText(spin.array), a.expr, a.key, a.op, a.sep) if computed else
+                job(Dampr, plan.MemoryText(spin.array), a.value, a.op, sep=a.sep, key_fields=K)).run())
 
     kernel_ms = min(m[1] for m in mem)
     res = {
@@ -410,6 +496,10 @@ def main():
                     "kernels_ms": {k: round(v, 3) for k, v in sorted(best[4].items())}})
         if a.value == "float" and a.op in ("sum", "mean"):
             res["sample_within_bound"] = within_bound(got, host, magnitudes(sample, a.sep, K), a.op)
+        if computed:
+            res.update({"expr": a.expr, "key": a.key})
+            if a.expr == "ratio" or a.op == "mean":
+                res["sample_within_bound"] = within_bound(got, host, host_mag, a.op)
     if K > 1:
         res.update({"key_fields": K, "fetch_to_frame_ms": round(1e3 * min(fetch_s[1:1 + a.reps]), 3)})
     if a.where != "none":
