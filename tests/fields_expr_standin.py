@@ -8,7 +8,7 @@ import math
 
 from fields_standin import M64, _int18, f64_bits, parse_f64
 from fields_tuple_standin import make_tuple_ctx
-from fields_where_standin import where
+from fields_where_standin import line_verdict
 from fields_ws_standin import WsLine
 
 I64_MIN, I64_MAX, LIM53 = -(1 << 63), (1 << 63) - 1, 1 << 53
@@ -128,15 +128,14 @@ def make_expr_ctx(free_bytes=1 << 30):
             st = self.st
             sep, kf, kind, vf, op = spec
             f = line.split() if sep == dev.FIELD_SEP_WS else line.split(bytes([sep]))
-            takes = len(line) < 4096 and all(0 < c < 0x80 for c in line) and (cr_is_data or b"\r" not in line)
-            verdict = where(f, preds) if preds and takes else True
-            if takes and verdict is False:
+            verdict = line_verdict(line, f, preds, cr_is_data)
+            if verdict is False:
                 if rec is not None:
                     self._put(rec, 0, 0)
                 else:
                     st["raw"] += 1
                 return
-            kv = expr_line(line, f, expr, spec) if takes and verdict is True else None
+            kv = expr_line(line, f, expr, spec) if verdict is True else None
             if kv is None:
                 self._hand_back(line, off, rec)
                 return

@@ -116,6 +116,40 @@ def json_where(m, preds, names):
     return True
 
 
+def json_line(line, spec, names, cr_is_data, preds):
+    """one line of a JSON scan: (outcome, flags). outcome is False (dropped), None (the host's) or (synth, key offset):
+    a line of the key's raw bytes, then 0x01 and the value's, which the plain scan reads as field 0 (the key) and
+    field 1 (the value, absent under FIELD_VAL_ONE), the key at that offset in the line; flags are the
+    DAMPR_TF_JSON_* flags the line raises"""
+    from dampr_b200 import device as dev
+    _sep, kf, kind, vf, op = spec
+    m = device_members(line, cr_is_data)
+    verdict = None if m is None else json_where(m, preds, names)
+    if verdict is not True:
+        return verdict, 0
+    flt = op in (dev.OP_SUM_F64, dev.OP_MIN_F64, dev.OP_MAX_F64)
+    k = m.get(names[kf])
+    v = None if vf == dev.FIELD_VAL_ONE else m.get(names[vf])
+    flags = 0
+    if k is not None and k[0] not in ((INT,) if kind == dev.FIELD_KEY_INT else (STR, ESC)):
+        flags |= dev.TF_JSON_KEY_KIND
+    if v is not None and v[0] != (FLOAT if flt else INT):
+        flags |= dev.TF_JSON_VAL_KIND
+    ok = k is not None and k[0] == (INT if kind == dev.FIELD_KEY_INT else STR)
+    if vf != dev.FIELD_VAL_ONE:
+        ok = ok and v is not None and v[0] in ((INT, FLOAT) if flt else (INT,))
+    if ok and kind == dev.FIELD_KEY_INT:
+        ok = _int18(k[1].encode()) is not None
+    if ok and vf != dev.FIELD_VAL_ONE:
+        raw = v[1].encode()
+        # float() of a JSON integer is float(int): "-0" is 0.0
+        val = (b"0" if raw == b"-0" and flt else raw)
+        ok = (parse_f64(val) if flt else _int18(val)) is not None
+    if not ok:
+        return None, flags
+    return (k[1].encode() + (b"" if vf == dev.FIELD_VAL_ONE else b"\x01" + val), k[2]), flags
+
+
 def make_json_ctx(free_bytes=1 << 30):
     """make_where_ctx(free_bytes) whose tables also take json_fields() and json_fields_records()"""
     from dampr_b200 import device as dev
@@ -147,41 +181,21 @@ def make_json_ctx(free_bytes=1 << 30):
                 pos = end + 1
 
         def _json_line(self, line, off, spec, names, cr_is_data, preds, rec):
-            _sep, kf, kind, vf, op = spec
-            m = device_members(line, cr_is_data)
-            verdict = None if m is None else json_where(m, preds, names)
-            if verdict is False:
+            _sep, _kf, kind, vf, op = spec
+            got, flags = json_line(line, spec, names, cr_is_data, preds)
+            self.st["flags"] |= flags
+            if got is False:
                 if rec is not None:
                     self._put(rec, 0, 0)
                 else:
                     self.st["raw"] += 1
                 return
-            if verdict is None:
-                self._hand_back(line, off, rec)
-                return
-            flt = op in (dev.OP_SUM_F64, dev.OP_MIN_F64, dev.OP_MAX_F64)
-            k = m.get(names[kf])
-            v = None if vf == dev.FIELD_VAL_ONE else m.get(names[vf])
-            if k is not None and k[0] not in ((INT,) if kind == dev.FIELD_KEY_INT else (STR, ESC)):
-                self.st["flags"] |= dev.TF_JSON_KEY_KIND
-            if v is not None and v[0] != (FLOAT if flt else INT):
-                self.st["flags"] |= dev.TF_JSON_VAL_KIND
-            ok = k is not None and k[0] == (INT if kind == dev.FIELD_KEY_INT else STR)
-            if vf != dev.FIELD_VAL_ONE:
-                ok = ok and v is not None and v[0] in ((INT, FLOAT) if flt else (INT,))
-            if ok and kind == dev.FIELD_KEY_INT:
-                ok = _int18(k[1].encode()) is not None
-            if ok and vf != dev.FIELD_VAL_ONE:
-                raw = v[1].encode()
-                # float() of a JSON integer is float(int): "-0" is 0.0
-                val = (b"0" if raw == b"-0" and flt else raw)
-                ok = (parse_f64(val) if flt else _int18(val)) is not None
-            if not ok:
+            if got is None:
                 self._hand_back(line, off, rec)
                 return
             # the plain stand-in over a line of the key's and the value's raw bytes, the key first at its own offset
-            synth = k[1].encode() + (b"" if vf == dev.FIELD_VAL_ONE else b"\x01" + val)
-            Plain._line(self, synth, off + k[2], b"\x01", 0, kind, dev.FIELD_VAL_ONE if vf == dev.FIELD_VAL_ONE
+            synth, k_off = got
+            Plain._line(self, synth, off + k_off, b"\x01", 0, kind, dev.FIELD_VAL_ONE if vf == dev.FIELD_VAL_ONE
                         else 1, op, cr_is_data, rec)
 
     ctx.table = lambda log2: JsonTable(ctx, log2)

@@ -106,6 +106,24 @@ def _int18(b):
     return -int(s) if b[:1] == b"-" else int(s)
 
 
+def device_takes(line, cr_is_data):
+    """the header's rule of the lines a field scan may take: under 4 KB, ASCII without NUL, no text-mode '\\r'"""
+    return len(line) < 4096 and all(0 < c < 0x80 for c in line) and (cr_is_data or b"\r" not in line)
+
+
+def plain_line(line, f, kf, kind, vf, flt, cr_is_data):
+    """(key, value) the plain scan folds for a line whose fields are f (bytes), or None for a line it hands to the
+    host: a str key is bytes, an int key an int; the value 1 (vf FIELD_VAL_ONE), a float (flt) or an int"""
+    from dampr_b200 import device as dev
+    ok = device_takes(line, cr_is_data) and -len(f) <= kf < len(f) and \
+        (vf == dev.FIELD_VAL_ONE or -len(f) <= vf < len(f))
+    if not ok:
+        return None
+    v = 1 if vf == dev.FIELD_VAL_ONE else parse_f64(f[vf]) if flt else _int18(f[vf])
+    k = _int18(f[kf]) if kind == dev.FIELD_KEY_INT else f[kf]
+    return None if v is None or k is None else (k, v)
+
+
 def f64_bits(v):
     return struct.unpack("<Q", struct.pack("<d", v))[0]
 
@@ -162,14 +180,9 @@ def make_ctx(free_bytes=1 << 30):
         def _line(self, line, off, sep, kf, kind, vf, op, cr_is_data, rec):
             st = self.st
             f = line.split(sep)
-            ok = len(line) < 4096 and all(0 < c < 0x80 for c in line) and (cr_is_data or b"\r" not in line)
-            ok = ok and -len(f) <= kf < len(f) and (vf == dev.FIELD_VAL_ONE or -len(f) <= vf < len(f))
             flt = op in (dev.OP_SUM_F64, dev.OP_MIN_F64, dev.OP_MAX_F64)
-            v = None if not ok else 1 if vf == dev.FIELD_VAL_ONE else parse_f64(f[vf]) if flt else _int18(f[vf])
-            k = f[kf] if ok else None
-            if ok and kind == dev.FIELD_KEY_INT:
-                k = _int18(k)
-            if not ok or v is None or k is None:
+            kv = plain_line(line, f, kf, kind, vf, flt, cr_is_data)
+            if kv is None:
                 if len(line) > 0xFFFF:
                     st["flags"] |= dev.TF_LONGLINE
                 elif len(self.fb) < (1 << 16):
@@ -180,6 +193,7 @@ def make_ctx(free_bytes=1 << 30):
                 if rec is not None:
                     self._put(rec, 0, 0)
                 return
+            k, v = kv
             st["lines"] += 1
             st["folded"] += 1
             if flt and v == 0 and math.copysign(1.0, v) < 0:

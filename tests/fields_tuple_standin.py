@@ -5,7 +5,7 @@ exactly like the whitespace stand-in's.
 
 It also holds a plain-Python statement of the tuple key code, which the GPU tests compare the kernel's codes with."""
 from fields_standin import M64, _int18, f64_bits, parse_f64
-from fields_where_standin import where
+from fields_where_standin import line_verdict
 from fields_ws_standin import WsLine, make_ws_ctx
 
 SEED = 0x243F6A8885A308D3
@@ -31,6 +31,22 @@ def tuple_code(parts):
         h2 = ((h2 ^ c) * 0x85EBCA6B + 0x9E3779B9) & M32
         h2 = ((h2 << 13) | (h2 >> 19)) & M32
     return mix64(((h1 << 32) | h2) ^ ((len(fed) * 0x9E3779B97F4A7C15) & M64)) | (1 << 63)
+
+
+def tuple_line(line, f, spec, keys, cr_is_data, preds):
+    """one line of a tuple-key scan whose fields are f: False (dropped), None (the host's) or (components, value), a
+    str component bytes and an int() one an int"""
+    from dampr_b200 import device as dev
+    _sep, _kf, _kind, vf, op = spec
+    verdict = line_verdict(line, f, preds, cr_is_data)
+    if verdict is not True:
+        return verdict
+    flt = op in (dev.OP_SUM_F64, dev.OP_MIN_F64, dev.OP_MAX_F64)
+    if not all(-len(f) <= i < len(f) for i, _k in keys) or not (vf == dev.FIELD_VAL_ONE or -len(f) <= vf < len(f)):
+        return None
+    v = 1 if vf == dev.FIELD_VAL_ONE else parse_f64(f[vf]) if flt else _int18(f[vf])
+    parts = [f[i] if k == dev.FIELD_KEY_STR else _int18(f[i]) for i, k in keys]
+    return None if v is None or None in parts else (parts, v)
 
 
 def make_tuple_ctx(free_bytes=1 << 30):
@@ -71,22 +87,18 @@ def make_tuple_ctx(free_bytes=1 << 30):
             st = self.st
             sep, _kf, _kind, vf, op = spec
             f = line.split() if sep == dev.FIELD_SEP_WS else line.split(bytes([sep]))
-            takes = len(line) < 4096 and all(0 < c < 0x80 for c in line) and (cr_is_data or b"\r" not in line)
-            verdict = where(f, preds) if preds and takes else True
-            if takes and verdict is False:
+            got = tuple_line(line, f, spec, keys, cr_is_data, preds)
+            if got is False:
                 if rec is not None:
                     self._put(rec, 0, 0)
                 else:
                     st["raw"] += 1
                 return
-            flt = op in (dev.OP_SUM_F64, dev.OP_MIN_F64, dev.OP_MAX_F64)
-            ok = takes and verdict is True and all(-len(f) <= i < len(f) for i, _k in keys) and \
-                (vf == dev.FIELD_VAL_ONE or -len(f) <= vf < len(f))
-            v = None if not ok else 1 if vf == dev.FIELD_VAL_ONE else parse_f64(f[vf]) if flt else _int18(f[vf])
-            parts = [f[i] if k == dev.FIELD_KEY_STR else _int18(f[i]) for i, k in keys] if ok else [None]
-            if v is None or None in parts:
+            if got is None:
                 self._hand_back(line, off, rec)
                 return
+            parts, v = got
+            flt = op in (dev.OP_SUM_F64, dev.OP_MIN_F64, dev.OP_MAX_F64)
             st["lines"] += 1
             st["folded"] += 1
             if flt and v == 0 and str(v).startswith("-"):

@@ -5,7 +5,7 @@ dampr_text_fields_records (include/dampr_b200.h): the tests of `filter(...)` in 
 Per line the device can take (ASCII, no NUL, no text-mode '\\r', under 4 KB), the predicates are evaluated in order:
 the first false one drops the line (a hole in record mode, stats[6] in table mode), the first one the device cannot
 decide hands the line back as a fallback line, and a line that passes all of them is the plain stand-in's."""
-from fields_standin import _int18, make_ctx, parse_f64
+from fields_standin import _int18, device_takes, make_ctx, parse_f64
 
 _CMPS = [lambda x, c: x == c, lambda x, c: x != c, lambda x, c: x < c, lambda x, c: x <= c, lambda x, c: x > c,
          lambda x, c: x >= c]
@@ -35,6 +35,14 @@ def where(f, preds):
     return True
 
 
+def line_verdict(line, f, preds, cr_is_data):
+    """the WHERE rule of one line whose fields are f: False (dropped), None (the host's: a line the device does not
+    take, or a predicate it cannot decide) or True (the key and value decide)"""
+    if not device_takes(line, cr_is_data):
+        return None
+    return where(f, preds) if preds else True
+
+
 def make_where_ctx(free_bytes=1 << 30):
     """make_ctx(free_bytes) whose tables also take the `preds` of fields() and fields_records()"""
     from dampr_b200 import device as dev
@@ -55,8 +63,7 @@ def make_where_ctx(free_bytes=1 << 30):
             Base.fields_records(self, tb, lo, hi, spec, kv, cr_is_data)
 
         def _line(self, line, off, sep, kf, kind, vf, op, cr_is_data, rec):
-            takes = len(line) < 4096 and all(0 < c < 0x80 for c in line) and (cr_is_data or b"\r" not in line)
-            verdict = where(line.split(sep), self._preds) if self._preds and takes else True
+            verdict = line_verdict(line, line.split(sep), self._preds, cr_is_data)
             if verdict is False:      # dropped: a hole in record mode, counted in stats[6] in table mode
                 if rec is not None:
                     self._put(rec, 0, 0)
