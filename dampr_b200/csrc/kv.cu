@@ -426,6 +426,7 @@ leaf_sort_kernel(const ulonglong2 *__restrict__ data, ulonglong2 *__restrict__ o
 __global__ void single_group_reduce_kernel(const ulonglong2 *__restrict__ data, u64 start, u64 n, int op,
                                            ulonglong2 *__restrict__ out_rec) {
     __shared__ u64 part[32];
+    __shared__ u32 parth[32];  // the warp's partial holds at least one record
     u64 acc = 0;
     bool have = false;
     // FIRST/LAST depend on order: handled by thread 0 directly
@@ -437,15 +438,36 @@ __global__ void single_group_reduce_kernel(const ulonglong2 *__restrict__ data, 
         return;
     }
     if (op == DAMPR_OP_SUM_F64) {
-        // deterministic: fixed strided partition + tree
+        // deterministic: fixed strided partition + tree. Every partial starts from its first value and empty
+        // partials are skipped, never added as +0.0: a group of -0.0 values sums to -0.0, as in a left fold
         double a = 0.0;
-        for (u64 i = threadIdx.x; i < n; i += blockDim.x) a += __longlong_as_double((long long)data[start + i].y);
-        for (int d = 16; d > 0; d >>= 1) a += __shfl_down_sync(0xFFFFFFFFu, a, d);
-        if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = (u64)__double_as_longlong(a);
+        for (u64 i = threadIdx.x; i < n; i += blockDim.x) {
+            const double v = __longlong_as_double((long long)data[start + i].y);
+            a = have ? a + v : v;
+            have = true;
+        }
+        for (int d = 16; d > 0; d >>= 1) {
+            const double o = __shfl_down_sync(0xFFFFFFFFu, a, d);
+            const u32 oh = __shfl_down_sync(0xFFFFFFFFu, (u32)have, d);
+            if (oh) {
+                a = have ? a + o : o;
+                have = true;
+            }
+        }
+        if ((threadIdx.x & 31) == 0) {
+            part[threadIdx.x >> 5] = (u64)__double_as_longlong(a);
+            parth[threadIdx.x >> 5] = have;
+        }
         __syncthreads();
         if (threadIdx.x == 0) {
             double t = 0.0;
-            for (u32 w = 0; w < blockDim.x / 32; ++w) t += __longlong_as_double((long long)part[w]);
+            bool th = false;
+            for (u32 w = 0; w < blockDim.x / 32; ++w)
+                if (parth[w]) {
+                    const double pw = __longlong_as_double((long long)part[w]);
+                    t = th ? t + pw : pw;
+                    th = true;
+                }
             *out_rec = make_ulonglong2(data[start].x, (u64)__double_as_longlong(t));
         }
         return;
@@ -464,7 +486,6 @@ __global__ void single_group_reduce_kernel(const ulonglong2 *__restrict__ data, 
             have = true;
         }
     }
-    __shared__ u32 parth[32];
     if ((threadIdx.x & 31) == 0) {
         part[threadIdx.x >> 5] = acc;
         parth[threadIdx.x >> 5] = have;

@@ -899,8 +899,9 @@ class FieldScan(TextScan):
         """raise NotLowerable when a host line's key or value would give the device's column another type"""
 
     def _record_sums(self, codes, n):
-        """per table key code (in `codes` order): the sum of its records' values, folded in line order by the stable
-        sort + segmented reduce (float64 under OP_SUM_F64, else int64)"""
+        """per table key code (in `codes` order): the sum of its records' values by the stable sort + segmented reduce
+        (float64 under OP_SUM_F64, else int64): in line order for a key of at most 4096 lines, by the fixed strided
+        tree of single_group_reduce_kernel for a larger one"""
         # dampr_kv_sort_reduce allocates its scratch copy at the buffer's capacity and an output of n records
         if 16 * (self._rec_cap + n) > self._free_bytes():
             raise NotLowerable("the sort scratch of the field records exceeds free device memory")

@@ -116,8 +116,9 @@ def test_sort_narrow_cluster_next_to_the_whole_range(ctx, n):
 
 # ---- folds ---------------------------------------------------------------------------------------------------
 def fold_values(op, rng, n):
-    """values in the domain the planner sends to each op (runner.py, plan.py): NaN- and -0.0-free floats for MIN /
-    MAX_F64, finite floats for SUM_F64, int64 extremes for MIN / MAX_I64, sums that stay in 64 bits"""
+    """values for each op: NaN- and -0.0-free floats for MIN / MAX_F64 (the planner sends those to the host), finite
+    floats for SUM_F64, int64 extremes for MIN / MAX_I64, sums that stay in 64 bits. SUM_F64 also receives -0.0, +-inf
+    and NaN from the planner; those, and the bit-exact checks, are in test_gpu_float_sums.py"""
     if op in (dev.OP_MIN_F64, dev.OP_MAX_F64):
         pool = np.array([0.0, np.inf, -np.inf, 5e-324, -5e-324, 2.225073858507201e-308, -2.5, 1.7976931348623157e308,
                          -1.7976931348623157e308, 3.0])
