@@ -39,7 +39,9 @@
 // Predicate j owns bound slot j; the separator walk that finds the key and value also finds every predicate's
 // field, the slots unrolled at compile time so the bounds stay in registers. The predicates are then evaluated in
 // chain order: the first false one drops the line before its key or value is parsed (a hole in record mode); one
-// the device cannot decide sends the line to the host, whose Python filters decide or raise.
+// the device cannot decide sends the line to the host, whose Python filters decide or raise. A program with `and` /
+// `or` / `not` (WhereProg, behind the parameters the plain builds read) evaluates every leaf to T, F or U and folds
+// them left-sequentially, as Python's short circuit does (where_program); a leaf may also read the whole line.
 //
 // WS (`line.split()`, DAMPR_FIELD_SEP_WS, a compile-time parameter, so the single-byte scans compile as before): the
 // separator mask becomes the str.split() whitespace mask (0x09-0x0D, 0x1C-0x20; '\r' only reaches it under
@@ -113,14 +115,31 @@ struct PredSlot {
     u8 first, n;         // constants c[first, first + n)
 };
 
+// a WHERE program's entries: leaf j (< P_MAX) or a connective
+enum : u8 { W_AND = 0x80, W_OR = 0x81, W_NOT = 0x82 };
+
 // the predicates of a WHERE scan, passed by value in the kernel parameters (4 KB limit)
 struct WhereView {
-    PredSlot p[P_MAX];
-    long long c[DAMPR_PRED_MAX_CONSTS];   // INT / NFIELDS values, the bits of an F64 constant, STR: offset << 32 | len
+    PredSlot p[P_MAX];                    // the leaves; leaf j owns bound slot j
+    long long c[DAMPR_PRED_MAX_CONSTS];   // INT / NFIELDS / LEN values, F64 constant bits, STR: offset << 32 | len
     u8 b[DAMPR_PRED_MAX_BYTES];           // STR constants
-    int n;
+    int n;                                // leaves
 };
-static_assert(sizeof(WhereView) + 256 <= 4096, "kernel parameters");
+
+// a WHERE program with connectives. It travels after the parameters a plain build reads (the tuple components, the
+// expression programs), so those keep their offsets and the plain builds their code.
+struct WhereProg {
+    int np;                               // entries of op; 0: the leaves are an AND chain
+    u8 op[P_MAX + DAMPR_PRED_MAX_OPS];    // postfix: leaf indices and W_AND / W_OR / W_NOT
+};
+
+// the parameter of the separator-byte, whitespace and JSON WHERE builds (fields_tiles finds `g` behind `v`, as it
+// finds a TupleWhere's members)
+struct Where {
+    WhereView v;
+    WhereProg g;
+};
+static_assert(sizeof(Where) + 256 <= 4096, "kernel parameters");
 
 struct SmemF {
     alignas(16) u8 text[F_WIN];
@@ -194,12 +213,68 @@ __device__ __forceinline__ int str_order(const WhereView &w, const u8 *p, u32 le
     return len < kl ? -1 : (len > kl ? 1 : 0);
 }
 
+// `s in p[0, len)` for a constant s of kl bytes: a scan of aligned words of the field in shared memory for s's first
+// byte, then a byte compare at each hit. O(len * kl) at worst (4 KB x 1 KB).
+__device__ __forceinline__ bool contains(const u8 *p, u32 len, const u8 *s, u32 kl) {
+    if (kl == 0) return true;
+    if (kl > len) return false;
+    const u32 a = (u32)(uintptr_t)p & 3u, hi = a + len - kl + 1;   // candidate starts: word bytes [a, hi)
+    const u8 *base = p - a;
+    const u32 k0 = s[0] * 0x01010101u;
+    for (u32 o = 0; o < hi; o += 4) {
+        u32 m = __vcmpeq4(*reinterpret_cast<const u32 *>(base + o), k0);
+        if (o == 0) m &= ~0u << (8 * a);
+        if (o + 4 > hi) m &= (1u << (8 * (hi - o))) - 1u;
+        while (m) {
+            const u32 b = ((u32)__ffs(m) - 1u) >> 3, i = o + b - a;
+            m &= ~(0xFFu << (8 * b));   // __vcmpeq4 sets all 8 bits of a hit
+            u32 j = 1;
+            while (j < kl && p[i + j] == s[j]) ++j;
+            if (j == kl) return true;
+        }
+    }
+    return false;
+}
+
+// p[0, len) holds a byte outside the str.split() whitespace class (`x.strip()` is truthy)
+__device__ __forceinline__ bool nonblank(const u8 *p, u32 len) {
+    const u32 a = (u32)(uintptr_t)p & 3u, hi = a + len;
+    const u8 *base = p - a;
+    for (u32 o = 0; o < hi; o += 4) {
+        u32 nl, ws, bd;
+        classify<true>(*reinterpret_cast<const u32 *>(base + o), 0u, true, nl, ws, bd);
+        u32 keep = 0x80808080u;
+        if (o == 0) keep &= ~0u << (8 * a);
+        if (o + 4 > hi) keep &= (1u << (8 * (hi - o))) - 1u;
+        if (~ws & keep) return true;
+    }
+    return false;
+}
+
 // one predicate over its field p[0, len) (nf: the line's field count): 1 true, 0 false, -1 for the host to decide
 // (no such field, or an int() / float() field the device does not parse exactly)
 __device__ __noinline__ int eval_pred(const WhereView &w, const PredSlot &pr, bool has, const u8 *p, u32 len,
                                       int nf) {
     if (pr.kind == DAMPR_PRED_NFIELDS) return cmp_holds(pr.cmp, nf < w.c[pr.first] ? -1 : nf > w.c[pr.first]);
     if (!has) return -1;   // IndexError in Python
+    if (pr.kind == DAMPR_PRED_LEN) return cmp_holds(pr.cmp, len < w.c[pr.first] ? -1 : len > w.c[pr.first]);
+    if (pr.kind == DAMPR_PRED_NONBLANK) return nonblank(p, len);
+    if (pr.cmp >= DAMPR_CMP_CONTAINS) {   // STR: substring, prefix, suffix
+        if (pr.cmp <= DAMPR_CMP_NOT_CONTAINS) {
+            const long long k = w.c[pr.first];
+            return contains(p, len, w.b + (k >> 32), (u32)k) == (pr.cmp == DAMPR_CMP_CONTAINS);
+        }
+        for (int i = pr.first; i < pr.first + pr.n; ++i) {
+            const u8 *s = w.b + (w.c[i] >> 32);
+            const u32 kl = (u32)w.c[i];
+            if (kl > len) continue;
+            const u8 *q = pr.cmp == DAMPR_CMP_STARTS ? p : p + len - kl;
+            u32 j = 0;
+            while (j < kl && q[j] == s[j]) ++j;
+            if (j == kl) return 1;
+        }
+        return 0;
+    }
     const bool in = pr.cmp == DAMPR_CMP_IN || pr.cmp == DAMPR_CMP_NOT_IN;
     bool r = false;
     if (pr.kind == DAMPR_PRED_F64) {
@@ -226,6 +301,37 @@ __device__ __noinline__ int eval_pred(const WhereView &w, const PredSlot &pr, bo
             r = (u32)w.c[i] == len && str_order(w, p, len, w.c[i]) == 0;
     }
     return r == (pr.cmp == DAMPR_CMP_IN);
+}
+
+// the verdict of a WHERE program (1 T, 0 F, -1 U) from its leaves' results: bit j of t / u says leaf j is T / U.
+// A stack of three-valued bits (top at bit 0) under left-sequential logic, Python's short circuit: `a and b` is a
+// when a is F or U, else b; `a or b` is a when a is T or U, else b; `not` keeps U. The values left are ANDed bottom
+// first (one per filter call).
+__device__ __forceinline__ int where_program(const WhereProg &g, u32 t, u32 u) {
+    u32 st = 0, su = 0;
+    int d = 0;
+    for (int k = 0; k < g.np; ++k) {
+        const u32 op = g.op[k];
+        if (op < (u32)P_MAX) {
+            st = (st << 1) | ((t >> op) & 1u);
+            su = (su << 1) | ((u >> op) & 1u);
+            ++d;
+        } else if (op == W_NOT) {
+            st ^= ~su & 1u;
+        } else {
+            const u32 bt = st & 1u, bu = su & 1u;
+            st >>= 1;
+            su >>= 1;
+            --d;
+            if (!(su & 1u) && (st & 1u) == (op == W_AND ? 1u : 0u)) {   // a does not decide: the result is b
+                st = (st & ~1u) | bt;
+                su = (su & ~1u) | bu;
+            }
+        }
+    }
+    const u32 open = ~st & ((1u << d) - 1u);   // the values that are not T
+    if (!open) return 1;
+    return (su >> (31 - __clz(open))) & 1u ? -1 : 0;
 }
 
 // ---- JSON lines ------------------------------------------------------------------------------------------------
@@ -454,11 +560,13 @@ struct TupleView {
     int n;
 };
 
-// the parameters of a tuple-key build: its predicates (n = 0 in a plain build) and components. fields_tiles takes the
-// address of `where` (a pointer to the first member of this standard-layout struct) and finds `tup` behind it.
+// the parameters of a tuple-key build: its predicates (n = 0 in a plain build), components and WHERE program.
+// fields_tiles takes the address of `where` (a pointer to the first member of this standard-layout struct) and finds
+// `tup` and `prog` behind it.
 struct TupleWhere {
     WhereView where;
     TupleView tup;
+    WhereProg prog;
 };
 
 // ---- computed keys and values ----------------------------------------------------------------------------------
@@ -479,11 +587,12 @@ struct ExprView {
 };
 
 // the parameters of an expression build: fields_tiles finds `tup` (the load slots) where a tuple build does, and `ex`
-// behind it
+// and `prog` behind it
 struct ExprWhere {
     WhereView where;
     TupleView tup;
     ExprView ex;
+    WhereProg prog;
 };
 
 // the value of load slot j (unrolled: the slots stay in registers)
@@ -931,24 +1040,34 @@ __device__ __forceinline__ void json_fold(const u8 *t, u32 q, u32 end, u64 g0, c
     }
     if constexpr (WHERE) {
         const WhereView &wh = *where;
+        const WhereProg *prog = &reinterpret_cast<const Where *>(where)->g;
         int verdict = 1;
+        u32 lt = 0, lu = 0;   // a program's leaf results: T / U bits
 #pragma unroll
         for (int j = 0; j < P_MAX; ++j) {
-            if (j < wh.n && verdict == 1) {
+            if (j < wh.n && (verdict == 1 || prog->np)) {
                 const PredSlot &pr = wh.p[j];
                 const u32 ty = (mt >> (4 * pr.field)) & 0xFu;
+                int r;
                 if (pr.kind == DAMPR_PRED_MEMBER) {
-                    verdict = (ty != JT_NONE) == (pr.cmp == DAMPR_CMP_IN);
+                    r = (ty != JT_NONE) == (pr.cmp == DAMPR_CMP_IN);
                 } else {
                     // a member of another type than the constant's, or a missing one: the host's filter decides
-                    const bool has = pr.kind == DAMPR_PRED_STR ? ty == JT_STR
-                                     : pr.kind == DAMPR_PRED_INT ? ty == JT_INT
-                                                                 : (ty == JT_INT || ty == JT_FLOAT);
+                    const bool has = pr.kind == DAMPR_PRED_INT ? ty == JT_INT
+                                     : pr.kind == DAMPR_PRED_F64 ? (ty == JT_INT || ty == JT_FLOAT)
+                                                                 : ty == JT_STR;
                     const u32 b = member_bounds<JM>(mb, pr.field);
-                    verdict = eval_pred(wh, pr, has, t + (b & 0xFFFFu), (b >> 16) - (b & 0xFFFFu), 0);
+                    r = eval_pred(wh, pr, has, t + (b & 0xFFFFu), (b >> 16) - (b & 0xFFFFu), 0);
+                }
+                if (prog->np) {
+                    lt |= (u32)(r == 1) << j;
+                    lu |= (u32)(r < 0) << j;
+                } else {
+                    verdict = r;
                 }
             }
         }
+        if (prog->np) verdict = where_program(*prog, lt, lu);
         dropped = verdict == 0;
         to_host = verdict < 0;
         if (verdict != 1) return;
@@ -1178,7 +1297,8 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                     u32 ks = (!WS && ki == 0) ? q : 0xFFFFFFFFu, ke = (ki == nf - 1) ? end : 0xFFFFFFFFu;
                     u32 vs = (!WS && vi == 0) ? q : 0xFFFFFFFFu, ve = (vi == nf - 1) ? end : 0xFFFFFFFFu;
                     int need = max(ki, vi) + 1;   // separators to visit
-                    // WHERE: predicate j's field is pi[j] (-1: none, IndexError in Python), its bounds [ps[j], pe[j])
+                    // WHERE: predicate j's field is pi[j] (-1: none, IndexError in Python; -2: the whole line, which
+                    // takes no bound slot), its bounds [ps[j], pe[j])
                     int pi[WHERE ? P_MAX : 1];
                     u32 ps[WHERE ? P_MAX : 1], pe[WHERE ? P_MAX : 1];
                     if constexpr (WHERE) {
@@ -1186,13 +1306,14 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
 #pragma unroll
                         for (int j = 0; j < P_MAX; ++j) {
                             int i = -1;
-                            if (j < wh.n && wh.p[j].kind != DAMPR_PRED_NFIELDS) {
+                            const bool line = j < wh.n && wh.p[j].field == DAMPR_FIELD_LINE;
+                            if (j < wh.n && wh.p[j].kind != DAMPR_PRED_NFIELDS && !line) {
                                 i = wh.p[j].field < 0 ? wh.p[j].field + nf : wh.p[j].field;
                                 if (i >= nf) i = -1;
                             }
-                            pi[j] = i < 0 ? -1 : i;
-                            ps[j] = !WS && pi[j] == 0 ? q : 0xFFFFFFFFu;
-                            pe[j] = pi[j] == nf - 1 ? end : 0xFFFFFFFFu;
+                            pi[j] = line ? -2 : i < 0 ? -1 : i;
+                            ps[j] = line || (!WS && pi[j] == 0) ? q : 0xFFFFFFFFu;
+                            pe[j] = line || pi[j] == nf - 1 ? end : 0xFFFFFFFFu;
                             need = max(need, pi[j] + 1);
                         }
                     }
@@ -1295,12 +1416,26 @@ __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n,
                     if constexpr (WHERE) {
                         // chain order: the first false predicate drops the line, the first undecided one (and a
                         // missing key or value field behind predicates that all hold) is the host's
+                        // (a program evaluates every leaf, then folds their results)
                         const WhereView &wh = *where;
+                        const WhereProg *prog = EXPR ? &reinterpret_cast<const ExprWhere *>(where)->prog
+                                                : TUP ? &reinterpret_cast<const TupleWhere *>(where)->prog
+                                                      : &reinterpret_cast<const Where *>(where)->g;
                         int verdict = 1;
+                        u32 lt = 0, lu = 0;
 #pragma unroll
-                        for (int j = 0; j < P_MAX; ++j)
-                            if (j < wh.n && verdict == 1)
-                                verdict = eval_pred(wh, wh.p[j], pi[j] >= 0, s.text + ps[j], pe[j] - ps[j], nf);
+                        for (int j = 0; j < P_MAX; ++j) {
+                            if (j < wh.n && (verdict == 1 || prog->np)) {
+                                const int r = eval_pred(wh, wh.p[j], pi[j] != -1, s.text + ps[j], pe[j] - ps[j], nf);
+                                if (prog->np) {
+                                    lt |= (u32)(r == 1) << j;
+                                    lu |= (u32)(r < 0) << j;
+                                } else {
+                                    verdict = r;
+                                }
+                            }
+                        }
+                        if (prog->np) verdict = where_program(*prog, lt, lu);
                         dropped = verdict == 0;
                         to_host = verdict < 0 || (verdict == 1 && kv_missing);
                     }
@@ -1456,9 +1591,9 @@ text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, F
 template <int VK, int MODE, bool WHERE, bool WS>
 __global__ void __launch_bounds__(F_THREADS)
 text_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv,
-                   const __grid_constant__ WhereView where) {
+                   const __grid_constant__ Where where) {
     static_assert(WHERE, "a plain scan takes no predicates");
-    fields_tiles<VK, MODE, true, WS>(text, n, own_lo, own_hi, tab, rv, &where);
+    fields_tiles<VK, MODE, true, WS>(text, n, own_lo, own_hi, tab, rv, &where.v);
 }
 
 // the JSON-lines builds: the member names (and a WHERE scan's predicates) read in place from the parameters. The
@@ -1473,10 +1608,10 @@ text_json_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_
 template <int VK, int MODE>
 __global__ void __launch_bounds__(F_THREADS, 4)
 text_json_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv,
-                        const __grid_constant__ JsonView json, const __grid_constant__ WhereView where) {
-    fields_tiles<VK, MODE, true, false, true>(text, n, own_lo, own_hi, tab, rv, &where, &json);
+                        const __grid_constant__ JsonView json, const __grid_constant__ Where where) {
+    fields_tiles<VK, MODE, true, false, true>(text, n, own_lo, own_hi, tab, rv, &where.v, &json);
 }
-static_assert(sizeof(WhereView) + sizeof(JsonView) + 256 <= 4096, "kernel parameters");
+static_assert(sizeof(Where) + sizeof(JsonView) + 256 <= 4096, "kernel parameters");
 
 // the tuple-key builds (plain and WHERE) of the separator-byte and whitespace scans: the components (and the
 // predicates, unused by a plain build) read in place from the parameters. As for the JSON builds, saying that the
@@ -1506,7 +1641,7 @@ static_assert(sizeof(ExprWhere) + 256 <= 4096, "kernel parameters");
 // expression build over the load slots *tk and the programs *xe
 template <int VK, int MODE, bool WHERE = false, bool WS = false, bool JSON = false, bool TUP = false>
 int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const FieldsView &tv, const RecView &rv,
-                  int timer, const WhereView *wh = nullptr, const JsonView *jv = nullptr,
+                  int timer, const Where *wh = nullptr, const JsonView *jv = nullptr,
                   const TupleView *tk = nullptr, const ExprView *xe = nullptr) {
     const size_t smem = sizeof(SmemF);
     const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
@@ -1515,7 +1650,10 @@ int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, con
     if (xe) {
         if constexpr (!JSON && !TUP && MODE != M_COUNT) {
             ExprWhere xw{};
-            if (wh) xw.where = *wh;
+            if (wh) {
+                xw.where = wh->v;
+                xw.prog = wh->g;
+            }
             xw.tup = *tk;
             xw.ex = *xe;
             void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, ExprWhere) =
@@ -1526,7 +1664,10 @@ int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, con
         }
     } else if constexpr (TUP) {
         TupleWhere tw{};
-        if (wh) tw.where = *wh;
+        if (wh) {
+            tw.where = wh->v;
+            tw.prog = wh->g;
+        }
         tw.tup = *tk;
         void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, TupleWhere) =
             text_fields_tuple_kernel<VK, MODE, WHERE, WS>;
@@ -1534,7 +1675,7 @@ int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, con
         ScopedTimer tm(ctx, timer);
         kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, tw);
     } else if constexpr (JSON && WHERE) {
-        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonView, WhereView) =
+        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonView, Where) =
             text_json_fields_kernel<VK, MODE>;
         CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         ScopedTimer tm(ctx, timer);
@@ -1545,7 +1686,7 @@ int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, con
         ScopedTimer tm(ctx, timer);
         kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *jv);
     } else if constexpr (WHERE) {
-        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, WhereView) =
+        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, Where) =
             text_fields_kernel<VK, MODE, true, WS>;
         CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         ScopedTimer tm(ctx, timer);
@@ -1562,28 +1703,54 @@ int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, con
 
 // the predicates of spec in kernel-parameter form; DAMPR_ERR_ARG for a kind, comparison or limit outside the header's
 // (json: the predicates of a JSON scan, whose fields index the nmembers members; DAMPR_PRED_MEMBER instead of NFIELDS)
-int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, WhereView &w, bool json = false, int nmembers = 0) {
-    ARG_CHECK(ctx, spec->npreds >= 0 && spec->npreds <= DAMPR_PRED_MAX, "npreds must be 0 .. DAMPR_PRED_MAX");
+int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, Where &wv, bool json = false, int nmembers = 0) {
+    ARG_CHECK(ctx, spec->npreds >= 0 && spec->npreds <= DAMPR_PRED_MAX + DAMPR_PRED_MAX_OPS,
+              "npreds must be 0 .. DAMPR_PRED_MAX + DAMPR_PRED_MAX_OPS");
     ARG_CHECK(ctx, spec->npreds == 0 || spec->preds != nullptr, "null preds");
-    w = WhereView{};
-    w.n = spec->npreds;
-    int nc = 0, nb = 0;
-    for (int j = 0; j < spec->npreds; ++j) {
-        const dampr_field_pred &p = spec->preds[j];
+    wv = Where{};
+    WhereView &w = wv.v;
+    WhereProg &g = wv.g;
+    int nc = 0, nb = 0, nops = 0, depth = 0;
+    for (int e = 0; e < spec->npreds; ++e) {
+        const dampr_field_pred &p = spec->preds[e];
+        if (p.kind >= DAMPR_PRED_AND && p.kind <= DAMPR_PRED_NOT) {
+            const int pops = p.kind == DAMPR_PRED_NOT ? 1 : 2;
+            ARG_CHECK(ctx, depth >= pops, "a connective finds fewer operands than it takes");
+            ARG_CHECK(ctx, p.n == 0, "a connective takes no constants");
+            ARG_CHECK(ctx, ++nops <= DAMPR_PRED_MAX_OPS, "more than DAMPR_PRED_MAX_OPS connectives");
+            depth -= pops - 1;
+            g.op[g.np++] = (u8)(W_AND + (p.kind - DAMPR_PRED_AND));
+            continue;
+        }
+        ARG_CHECK(ctx, w.n < DAMPR_PRED_MAX, "more than DAMPR_PRED_MAX predicates");
+        const int j = w.n++;
+        g.op[g.np++] = (u8)j;
+        ++depth;
         const bool in = p.cmp == DAMPR_CMP_IN || p.cmp == DAMPR_CMP_NOT_IN;
         const bool member = json && p.kind == DAMPR_PRED_MEMBER;
-        if (json) {
-            ARG_CHECK(ctx, p.kind >= DAMPR_PRED_STR && p.kind <= DAMPR_PRED_MEMBER && p.kind != DAMPR_PRED_NFIELDS,
+        const bool text = p.kind == DAMPR_PRED_LEN || p.kind == DAMPR_PRED_NONBLANK;   // of a str field only
+        const bool any = p.cmp == DAMPR_CMP_STARTS || p.cmp == DAMPR_CMP_ENDS;         // n constants, any match
+        if (p.field == DAMPR_FIELD_LINE) {
+            ARG_CHECK(ctx, !json, "a JSON scan has no line operand");
+            ARG_CHECK(ctx, p.kind == DAMPR_PRED_STR || text, "the line operand is a str");
+        } else if (json) {
+            ARG_CHECK(ctx, p.kind >= DAMPR_PRED_STR && p.kind <= DAMPR_PRED_NONBLANK && p.kind != DAMPR_PRED_NFIELDS,
                       "predicate kind of a JSON scan");
             ARG_CHECK(ctx, p.field >= 0 && p.field < nmembers, "a JSON predicate's field must index the members");
         } else {
-            ARG_CHECK(ctx, p.kind >= DAMPR_PRED_STR && p.kind <= DAMPR_PRED_NFIELDS, "predicate kind");
+            ARG_CHECK(ctx, p.kind >= DAMPR_PRED_STR && p.kind <= DAMPR_PRED_NONBLANK && p.kind != DAMPR_PRED_MEMBER,
+                      "predicate kind");
         }
-        ARG_CHECK(ctx, p.cmp >= DAMPR_CMP_EQ && p.cmp <= DAMPR_CMP_NOT_IN, "predicate comparison");
+        ARG_CHECK(ctx, p.cmp >= DAMPR_CMP_EQ && p.cmp <= DAMPR_CMP_ENDS, "predicate comparison");
         ARG_CHECK(ctx, !member || in, "DAMPR_PRED_MEMBER takes IN or NOT_IN");
         ARG_CHECK(ctx, !in || member || p.kind == DAMPR_PRED_STR || p.kind == DAMPR_PRED_INT,
                   "IN / NOT_IN take STR or INT");
-        ARG_CHECK(ctx, member ? p.n == 0 : in ? (p.n >= 1 && p.n <= DAMPR_PRED_MAX_CONSTS) : p.n == 1,
+        ARG_CHECK(ctx, p.cmp < DAMPR_CMP_CONTAINS || p.kind == DAMPR_PRED_STR, "CONTAINS .. ENDS take STR");
+        ARG_CHECK(ctx, p.kind != DAMPR_PRED_LEN || p.cmp <= DAMPR_CMP_GE, "LEN takes EQ .. GE");
+        ARG_CHECK(ctx, p.kind != DAMPR_PRED_NONBLANK || p.cmp == DAMPR_CMP_EQ, "NONBLANK takes EQ");
+        ARG_CHECK(ctx, member || p.kind == DAMPR_PRED_NONBLANK ? p.n == 0
+                       : in || any                          ? (p.n >= 1 && p.n <= DAMPR_PRED_MAX_CONSTS)
+                                                            : p.n == 1,
                   "predicate constant count");
         ARG_CHECK(ctx, nc + p.n <= DAMPR_PRED_MAX_CONSTS, "more than DAMPR_PRED_MAX_CONSTS predicate constants");
         w.p[j] = PredSlot{p.field, (u8)p.kind, (u8)p.cmp, (u8)nc, (u8)p.n};
@@ -1607,6 +1774,7 @@ int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, WhereView &w, bool
             }
         }
     }
+    if (!nops) g.np = 0;   // no connective: the leaves are the AND chain
     return DAMPR_OK;
 }
 
@@ -1619,7 +1787,7 @@ int check_fields_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own
                        (spec->sep > 0 && spec->sep < 0x80 && spec->sep != '\n' && spec->sep != '\r'),
               "separator must be DAMPR_FIELD_SEP_WS or an ASCII byte other than NUL, '\\n' and '\\r'");
     ARG_CHECK(ctx, spec->key_kind == DAMPR_FIELD_KEY_STR || spec->key_kind == DAMPR_FIELD_KEY_INT, "key kind");
-    WhereView w;
+    Where w;
     return where_view(ctx, spec, w);
 }
 
@@ -1650,7 +1818,7 @@ int check_json_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own_l
         jv.len[j] = (u8)m->len[j];
         off += m->len[j];
     }
-    WhereView w;
+    Where w;
     return where_view(ctx, spec, w, true, m->n);
 }
 
@@ -1666,7 +1834,7 @@ template <int VK, int MODE, bool WS>
 int launch_fold_sep(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
                     const FieldsView &tv, const RecView &rv, const TupleView *tk, const ExprView *xe = nullptr) {
     if (xe) {
-        WhereView w{};
+        Where w{};
         if (spec->npreds == 0)
             return launch_fields<VK, MODE, false, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, nullptr,
                                                       nullptr, tk, xe);
@@ -1679,7 +1847,7 @@ int launch_fold_sep(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, c
         return launch_fields<VK, MODE, false, WS, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS,
                                                                nullptr, nullptr, tk);
     }
-    WhereView w;
+    Where w;
     if (int r = where_view(ctx, spec, w)) return r;
     if (!tk) return launch_fields<VK, MODE, true, WS>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w);
     return launch_fields<VK, MODE, true, WS, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w,
@@ -1694,7 +1862,7 @@ int launch_json_fold(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, 
     if (spec->npreds == 0 && jv.n <= 2)
         return launch_fields<VK, MODE, false, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS,
                                                           nullptr, &jv);
-    WhereView w;
+    Where w;
     if (int r = where_view(ctx, spec, w, true, jv.n)) return r;
     return launch_fields<VK, MODE, true, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w, &jv);
 }

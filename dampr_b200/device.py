@@ -43,9 +43,11 @@ EXPR_MAX_OPS, EXPR_MAX_LOADS, EXPR_MAX_DEPTH, EXPR_MAX_CONSTS = 32, 4, 8, 16
 EXPR_NONE, EXPR_INT, EXPR_F64 = 0, 1, 2
 LOAD_INT, LOAD_F64, LOAD_LEN = 0, 1, 2
 # WHERE predicates of a field scan (dampr_field_pred): kinds, comparisons, limits per call
-PRED_STR, PRED_INT, PRED_F64, PRED_NFIELDS, PRED_MEMBER = range(5)
-CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_IN, CMP_NOT_IN = range(8)
-PRED_MAX, PRED_MAX_CONSTS, PRED_MAX_BYTES = 8, 64, 1024
+PRED_STR, PRED_INT, PRED_F64, PRED_NFIELDS, PRED_MEMBER, PRED_LEN, PRED_NONBLANK, PRED_AND, PRED_OR, PRED_NOT = range(10)
+CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE, CMP_IN, CMP_NOT_IN, CMP_CONTAINS, CMP_NOT_CONTAINS, CMP_STARTS, \
+    CMP_ENDS = range(12)
+PRED_MAX, PRED_MAX_CONSTS, PRED_MAX_BYTES, PRED_MAX_OPS = 8, 64, 1024, 8
+FIELD_LINE = -(1 << 31)   # a predicate's field that is the whole line
 
 KERNEL_NAMES = {
     1: "text_count", 2: "table_extract", 3: "text_verify", 4: "part_hist", 5: "part_scatter",
@@ -84,7 +86,8 @@ class FieldsSpec(C.Structure):
 def fields_spec(spec, cr_is_data, preds):
     """dampr_fields_spec of spec = (sep byte or FIELD_SEP_WS, key field, key kind, value field or FIELD_VAL_ONE, op)
     and the WHERE predicates preds = [(PRED_*, field, CMP_*, constants)]: constants a tuple of str (PRED_STR), int
-    (PRED_INT, PRED_NFIELDS) or one float (PRED_F64). The returned structure keeps its constant arrays alive."""
+    (PRED_INT, PRED_NFIELDS, PRED_LEN) or one float (PRED_F64), () for PRED_NONBLANK, PRED_MEMBER and the connectives
+    PRED_AND / PRED_OR / PRED_NOT of a postfix program. The returned structure keeps its constant arrays alive."""
     sep, kf, kind, vf, op = spec
     arr = (FieldPred * max(1, len(preds)))()
     keep = [arr]
@@ -98,7 +101,7 @@ def fields_spec(spec, cr_is_data, preds):
             ln = (C.c_uint32 * len(raw))(*map(len, raw))
             p.bytes, p.lens = C.cast(b, C.POINTER(C.c_uint8)), C.cast(ln, C.POINTER(C.c_uint32))
             keep += [b, ln]
-        else:
+        elif consts:
             v = (C.c_int64 * len(consts))(*map(int, consts))
             p.ints = C.cast(v, C.POINTER(C.c_int64))
             keep.append(v)

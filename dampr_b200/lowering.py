@@ -40,7 +40,7 @@ class E(object):
 
 
 # node kinds: arg(i) const(v) obj(pyobject) attr(e, name) call(f, [args]) bin(op, l, r) neg(e)
-#             sub(e, idx) tuple([items]) cmp(op, l, r)
+#             sub(e, idx) tuple([items]) cmp(op, l, r) and(l, r) or(l, r) not(e)
 _NULL = object()
 
 
@@ -71,11 +71,41 @@ def analyze(fn):
     nargs = code.co_argcount
     argnames = code.co_varnames[:nargs]
     stack = []
+    # `a and b` / `a or b` compile to <a> COPY 1; POP_JUMP_IF_FALSE | POP_JUMP_IF_TRUE L; POP_TOP; <b>, merging at L.
+    # CPython threads jumps, so several merges can share one L (a and (b or c)) or land on the next COPY ((a and b) or
+    # c): pending holds (L, op, a, stack depth) and the merges at L combine innermost first when L is reached.
+    pending = []
+    ins_list = _instructions(code)
     try:
-        for ins in _instructions(code):
+        for k, ins in enumerate(ins_list):
+            while pending and pending[-1][0] == ins.offset:
+                _at, bop, lhs, depth = pending.pop()
+                if len(stack) != depth + 1:
+                    return None
+                stack.append(E(bop, lhs, stack.pop()))
+            if pending and pending[-1][0] < ins.offset:
+                return None
             name = ins.opname
             if name in ("RESUME", "NOP", "COPY_FREE_VARS", "MAKE_CELL", "PRECALL", "CACHE"):
                 continue
+            if name == "COPY" and ins.arg == 1:
+                nxt = ins_list[k + 1] if k + 2 < len(ins_list) else None
+                if nxt is None or nxt.opname not in ("POP_JUMP_IF_FALSE", "POP_JUMP_IF_TRUE") or \
+                        ins_list[k + 2].opname != "POP_TOP" or not nxt.argval > nxt.offset or \
+                        (pending and nxt.argval > pending[-1][0]):
+                    return None
+                lhs = stack.pop()
+                pending.append((nxt.argval, "and" if nxt.opname == "POP_JUMP_IF_FALSE" else "or", lhs, len(stack)))
+                continue
+            if name in ("POP_JUMP_IF_FALSE", "POP_JUMP_IF_TRUE", "POP_TOP") and k >= 1 and \
+                    ins_list[k - 1 if name != "POP_TOP" else k - 2].opname == "COPY" and \
+                    ins_list[k - 1 if name != "POP_TOP" else k - 2].arg == 1:
+                continue   # the rest of a short-circuit pattern (taken above)
+            if name == "UNARY_NOT":
+                stack.append(E("not", stack.pop()))
+                continue
+            if pending and name in ("RETURN_VALUE", "RETURN_CONST"):
+                return None
             if name in ("LOAD_FAST", "LOAD_FAST_CHECK"):
                 if ins.argval not in argnames:
                     return None
@@ -375,12 +405,18 @@ def field_predicate(fn, record=None, whitespace=False):
     e = analyze(fn)
     if e is None or e.op != "cmp":
         return None
+    return _field_leaf(e, _record_of(record, whitespace))
+
+
+def _record_of(record, whitespace):
+    """record(x) of a filter over the line (record None: its own l.split(S)) or over the split record of sep record"""
     if record is None:
-        def rec(x):
-            return _split_sep(x, whitespace)
-    else:
-        def rec(x):
-            return record if _is_arg(x) else None
+        return lambda x: _split_sep(x, whitespace)
+    return lambda x: record if _is_arg(x) else None
+
+
+def _field_leaf(e, rec):
+    """field_predicate's result for the comparison tree e"""
     op, l, r = e.a, e.b, e.c
     if op in _FLIP and _pred_const(l)[0] and not _pred_const(r)[0]:
         op, l, r = _FLIP[op], r, l
@@ -511,6 +547,11 @@ def json_predicate(fn):
     e = analyze(fn)
     if e is None or e.op != "cmp":
         return None
+    return _json_leaf(e)
+
+
+def _json_leaf(e):
+    """json_predicate's result for the comparison tree e"""
     op, l, r = e.a, e.b, e.c
     if op in ("in", "not in") and _is_arg(r):
         ok, name = _const(l)
@@ -553,6 +594,191 @@ def json_predicate(fn):
         elif type(v) is not float:
             return None
     return kind, name, op, consts
+
+
+# ---- filter programs: and / or / not over leaves, string tests, whole-line tests ---------------------------------
+LINE = "line"                     # the index of a leaf whose operand is the whole line
+FIELD_LEN = "len"                 # len(X) op n
+FIELD_NONBLANK = "nonblank"       # X.strip() as a truth value
+STR_TESTS = ("contains", "not contains", "startswith", "endswith")
+PRED_MAX_OPS = 8                  # connectives per stage (DAMPR_PRED_MAX_OPS)
+
+
+def _str_consts(consts):
+    """consts if every member is a str whose UTF-8 bytes exist (no lone surrogate), else None"""
+    if not all(type(c) is str for c in consts):
+        return None
+    try:
+        for c in consts:
+            c.encode("utf-8")
+    except UnicodeEncodeError:
+        return None
+    return tuple(consts)
+
+
+def _str_leaf(e, operand):
+    """(op, kind, operand index, consts) for a string test over a str operand: S in X, S not in X, X.startswith(S),
+    X.endswith(S) (S a str, or for the last two a tuple of str: a list raises TypeError in Python), len(X) op n /
+    n op len(X), and X.strip() as a truth value; operand(x) gives X's index (a field, LINE, a member) or None"""
+    if e.op == "cmp" and e.a in ("in", "not in"):
+        ok, s = _pred_const(e.b)
+        i = operand(e.c)
+        if ok and i is not None and type(s) is str and _str_consts((s,)):
+            return "contains" if e.a == "in" else "not contains", FIELD_STR, i, (s,)
+        return None
+    if e.op == "cmp" and e.a in _FLIP:
+        op, l, r = e.a, e.b, e.c
+        if _pred_const(l)[0] and not _pred_const(r)[0]:
+            op, l, r = _FLIP[op], r, l
+        ok, n = _pred_const(r)
+        if ok and type(n) is int and isinstance(l, E) and l.op == "call" and _callee(l.a) is len and \
+                len(l.b) == 1 and -(1 << 63) <= n < (1 << 63):
+            i = operand(l.b[0])
+            return None if i is None else (op, FIELD_LEN, i, (n,))
+        return None
+    if e.op == "call" and isinstance(e.a, E) and e.a.op == "attr" and e.a.b in ("startswith", "endswith", "strip"):
+        i = operand(e.a.a)
+        if i is None:
+            return None
+        if e.a.b == "strip":
+            return (None, FIELD_NONBLANK, i, ()) if e.b == () else None
+        if len(e.b) != 1:
+            return None
+        ok, s = _pred_const(e.b[0])
+        if not ok:
+            return None
+        consts = _str_consts((s,)) if type(s) is str else \
+            _str_consts(s) if type(s) is tuple and 1 <= len(s) <= PRED_MAX_CONSTS else None
+        return None if consts is None else (e.a.b, FIELD_STR, i, consts)
+    return None
+
+
+def _program(e, leaf):
+    """postfix list of a filter's tree: leaf(x) of every leaf ("and" / "or" / "not" for the connectives), or None when
+    a leaf is not one, or the program passes the device's limits"""
+    out = []
+
+    def walk(x):
+        if not isinstance(x, E):
+            return False
+        if x.op in ("and", "or"):
+            if not (walk(x.a) and walk(x.b)):
+                return False
+            out.append(x.op)
+            return True
+        if x.op == "not":
+            if not walk(x.a):
+                return False
+            out.append("not")
+            return True
+        got = leaf(x)
+        if got is None:
+            return False
+        out.append(got)
+        return True
+
+    if not walk(e):
+        return None
+    return out if _within_limits(out) else None
+
+
+def _within_limits(prog):
+    """the leaves, connectives, constants and string bytes of a program (or a stage's) fit the device"""
+    leaves = [x for x in prog if not isinstance(x, str)]
+    strs = [c for x in leaves for c in x[-1] if type(c) is str]
+    return len(leaves) <= PRED_MAX and len(prog) - len(leaves) <= PRED_MAX_OPS and \
+        sum(len(x[-1]) for x in leaves) <= PRED_MAX_CONSTS and sum(len(c.encode("utf-8")) for c in strs) <= PRED_MAX_BYTES
+
+
+def filter_program(fn, record=None, whitespace=False):
+    """Device WHERE program of a `filter(fn)` in front of a field fold, or None: the postfix list of its leaves and
+    connectives ("and", "or", "not"), fn's body being and / or / not over leaves. A leaf is field_predicate's result
+    (sep, kind, index, op, constants) for field_predicate's shapes, and, with X a str field R[i] or (record None: fn
+    takes the line) the line itself (index LINE, sep None):
+      S in X, S not in X                op "contains" / "not contains", kind FIELD_STR, constants (S,)
+      X.startswith(S), X.endswith(S)    op "startswith" / "endswith", FIELD_STR, S a str or a tuple of str
+      len(X) op n                       kind FIELD_LEN, constants (n,), n an int (not a bool)
+      X.strip() as a truth value        kind FIELD_NONBLANK, op None, constants ()
+      X op S, X in K                    the line under field_predicate's str comparisons
+    The limits are the device's: PRED_MAX leaves, PRED_MAX_OPS connectives, PRED_MAX_CONSTS constants and
+    PRED_MAX_BYTES bytes of str constants. Bare truthiness (lambda l: l), `S in r` over the split record, a field
+    inside a str constant (r[0] in "abc"), conditional expressions and chained comparisons are None."""
+    if not (isinstance(fn, types.FunctionType) and fn.__code__.co_argcount == 1):
+        return None
+    e = analyze(fn)
+    if e is None:
+        return None
+    rec = _record_of(record, whitespace)
+
+    def operand(x):   # (sep, index) of a str operand
+        if record is None and _is_arg(x):
+            return None, LINE
+        p = _field_proj(x, rec)
+        return (p[2], p[1]) if p is not None and p[0] == FIELD_STR else None
+
+    def leaf(x):
+        if x.op == "cmp":
+            p = _field_leaf(x, rec)
+            if p is not None:
+                return p
+            if record is None and x.a in ("in", "not in") + tuple(_FLIP) and \
+                    (_is_arg(x.b) or (_is_arg(x.c) and x.a in _FLIP)):
+                line = _line_cmp(x)
+                if line is not None:
+                    return line
+        got = _str_leaf(x, operand)
+        if got is None:
+            return None
+        op, kind, (sep, i), consts = got
+        return sep, kind, i, op, consts
+
+    return _program(e, leaf)
+
+
+def _line_cmp(e):
+    """(None, FIELD_STR, LINE, op, constants) for the line l compared with str constants: l op S, S op l, l in K"""
+    op, l, r = e.a, e.b, e.c
+    if op in _FLIP and _pred_const(l)[0] and _is_arg(r):
+        op, l, r = _FLIP[op], r, l
+    ok, c = _pred_const(r)
+    if not ok or not _is_arg(l):
+        return None
+    if op in ("in", "not in"):
+        if type(c) not in (tuple, frozenset, set, list) or not 1 <= len(c) <= PRED_MAX_CONSTS:
+            return None
+        consts = _str_consts(tuple(c))
+    else:
+        consts = _str_consts((c,))
+    return None if consts is None else (None, FIELD_STR, LINE, op, consts)
+
+
+def json_filter_program(fn):
+    """Device WHERE program of a `filter(fn)` behind map(json.loads), or None: the postfix list of json_predicate's
+    leaves (kind, name, op, constants) and of the string tests of filter_program over a member M = r["m"] (the
+    member's name in place of an index; the device decides them on a string member without escapes only), with the
+    connectives "and", "or", "not" between them"""
+    if not (isinstance(fn, types.FunctionType) and fn.__code__.co_argcount == 1):
+        return None
+    e = analyze(fn)
+    if e is None:
+        return None
+
+    def operand(x):
+        m = _member(x)
+        return m[1] if m is not None and m[0] == FIELD_DATA else None
+
+    def leaf(x):
+        if x.op == "cmp":
+            p = _json_leaf(x)
+            if p is not None:
+                return p
+        got = _str_leaf(x, operand)
+        if got is None:
+            return None
+        op, kind, name, consts = got
+        return kind, name, op, consts
+
+    return _program(e, leaf)
 
 
 def field_index(fn):
@@ -725,6 +951,8 @@ def depends_on(e, argi, fields=None):
             return False
         if x.op == "arg":
             return x.a != argi
+        if x.op in ("and", "or", "not"):   # boolean structure is not followed
+            return False
         return all(walk(y) for y in (x.a, x.b, x.c) if y is not None)
 
     return out if walk(e) else None

@@ -1127,7 +1127,7 @@ def _match_text_count(stage, inputs):
 KEY_TUPLE = "tuple"   # the key kind of a field scan's spec whose key is a tuple of fields
 
 
-def _match_text_fields(stage, inputs):
+def _match_text_fields(stage, inputs, programs=False):
     """filter* [map(l.split(S) | l.split()) filter*] keyed(field key, 1 | int(field) | float(field)) +
     PartialReduceCombiner(+ | min | max), or mean()'s keyed(field key, (int(field) | float(field), 1)) + component-wise
     (+, +), over text, each filter one lowering.field_predicate on the key's separator: (sources, (sep byte or
@@ -1135,7 +1135,10 @@ def _match_text_fields(stage, inputs):
     key of field projections has key kind KEY_TUPLE and, as its key index, the components ((index, FIELD_KEY_STR |
     FIELD_KEY_INT), ...). A sixth element is the stage's computed key / value programs (lowering.text_fields_expr, in
     device.field_expr form) for the shapes text_fields_spec refuses, else None: the map may then also compute an
-    expression or a tuple of them (no filter may follow such a map), a key program's keys are FIELD_KEY_INT keys."""
+    expression or a tuple of them (no filter may follow such a map), a key program's keys are FIELD_KEY_INT keys.
+    With `programs` each filter may be a lowering.filter_program (and / or / not, string tests, whole-line tests): the
+    device predicates are then the stage's postfix program (_device_program), the same 4-tuples as without it when no
+    filter needs more than one leaf of field_predicate's shapes."""
     if not isinstance(stage, GMap) or len(inputs) != 1:
         return None
     src = _text_files(inputs[0])
@@ -1169,14 +1172,20 @@ def _match_text_fields(stage, inputs):
     preds = []
     for i, (k, o) in enumerate(ks[:-1]):
         if k == "filter":
-            p = lowering.field_predicate(o.fn, sep if at is not None and i > at else None, whitespace=True)
-            if p is not None and sep is None:   # a computed key and value that read no field: the filters' split
-                sep = p[0]
-            if p is None or p[0] != sep:
+            rec = sep if at is not None and i > at else None
+            p = lowering.field_predicate(o.fn, rec, whitespace=True)
+            prog = [p] if p is not None else lowering.filter_program(o.fn, rec, whitespace=True) if programs else None
+            if prog is None:
                 return None
-            preds.append(_device_pred(p))
-    if len(preds) > dev.PRED_MAX or sum(len(p[3]) for p in preds) > dev.PRED_MAX_CONSTS or \
-            sum(len(c.encode("utf-8")) for p in preds if p[0] == dev.PRED_STR for c in p[3]) > dev.PRED_MAX_BYTES:
+            for p in prog:
+                if isinstance(p, str) or p[2] == lowering.LINE:
+                    continue
+                if sep is None:   # a computed key and value that read no field: the filters' split
+                    sep = p[0]
+                if p[0] != sep:
+                    return None
+            preds += _device_program(prog)
+    if not _preds_fit(preds):
         return None
     binop = stage.options.get("binop")
     if mean:
@@ -1202,11 +1211,12 @@ def _match_text_fields(stage, inputs):
                  dev.FIELD_VAL_ONE if vi is None else vi), op, mean, tuple(preds), expr
 
 
-def _match_json_fields(stage, inputs):
+def _match_json_fields(stage, inputs, programs=False):
     """map(json.loads) filter* keyed(r["k"] | int(r["k"]), 1 | r["v"] | int(r["v"]) | float(r["v"])) +
     PartialReduceCombiner(+ | min | max), or mean()'s keyed(key, (value, 1)) + component-wise (+, +), over text, each
     filter one lowering.json_predicate: (sources, (FIELD_SEP_JSON, key member, key kind, value member or FIELD_VAL_ONE),
-    op, mean, device predicates, member names, (bare key, bare value)) or None"""
+    op, mean, device predicates, member names, (bare key, bare value)) or None. With `programs` each filter may be a
+    lowering.json_filter_program, as _match_text_fields takes filter programs."""
     if not isinstance(stage, GMap) or len(inputs) != 1:
         return None
     src = _text_files(inputs[0])
@@ -1235,14 +1245,17 @@ def _match_json_fields(stage, inputs):
     preds = []
     for _k, o in ks[1:-1]:
         p = lowering.json_predicate(o.fn)
-        if p is None:
+        prog = [p] if p is not None else lowering.json_filter_program(o.fn) if programs else None
+        if prog is None:
             return None
-        kind, name, cmp, consts = p
-        preds.append((dev.PRED_MEMBER if kind == lowering.FIELD_MEMBER else _PRED_KINDS[kind], member(name),
-                      _PRED_CMPS[cmp], consts))
-    if len(members) > dev.JSON_MAX_MEMBERS or len(preds) > dev.PRED_MAX or \
-            sum(len(p[3]) for p in preds) > dev.PRED_MAX_CONSTS or \
-            sum(len(c.encode("utf-8")) for p in preds if p[0] == dev.PRED_STR for c in p[3]) > dev.PRED_MAX_BYTES:
+        for p in prog:
+            if isinstance(p, str):
+                preds.append((_PRED_OPS[p], 0, dev.CMP_EQ, ()))
+                continue
+            kind, name, cmp, consts = p
+            preds.append((dev.PRED_MEMBER if kind == lowering.FIELD_MEMBER else _PRED_KINDS[kind], member(name),
+                          _PRED_CMPS.get(cmp, dev.CMP_EQ), consts))
+    if len(members) > dev.JSON_MAX_MEMBERS or not _preds_fit(preds):
         return None
     binop = stage.options.get("binop")
     if mean:
@@ -1260,15 +1273,32 @@ def _match_json_fields(stage, inputs):
 
 
 _PRED_KINDS = {lowering.FIELD_STR: dev.PRED_STR, lowering.FIELD_INT: dev.PRED_INT, lowering.FIELD_FLOAT: dev.PRED_F64,
-               lowering.FIELD_COUNT: dev.PRED_NFIELDS}
+               lowering.FIELD_COUNT: dev.PRED_NFIELDS, lowering.FIELD_LEN: dev.PRED_LEN,
+               lowering.FIELD_NONBLANK: dev.PRED_NONBLANK}
 _PRED_CMPS = {"==": dev.CMP_EQ, "!=": dev.CMP_NE, "<": dev.CMP_LT, "<=": dev.CMP_LE, ">": dev.CMP_GT, ">=": dev.CMP_GE,
-              "in": dev.CMP_IN, "not in": dev.CMP_NOT_IN}
+              "in": dev.CMP_IN, "not in": dev.CMP_NOT_IN, "contains": dev.CMP_CONTAINS,
+              "not contains": dev.CMP_NOT_CONTAINS, "startswith": dev.CMP_STARTS, "endswith": dev.CMP_ENDS}
+_PRED_OPS = {"and": dev.PRED_AND, "or": dev.PRED_OR, "not": dev.PRED_NOT}
 
 
 def _device_pred(p):
-    """(PRED_*, field, CMP_*, constants) of a lowering.field_predicate"""
+    """(PRED_*, field, CMP_*, constants) of a lowering.field_predicate or a filter_program leaf"""
     _sep, kind, i, op, consts = p
-    return _PRED_KINDS[kind], 0 if i is None else i, _PRED_CMPS[op], consts
+    return _PRED_KINDS[kind], dev.FIELD_LINE if i == lowering.LINE else 0 if i is None else i, \
+        _PRED_CMPS.get(op, dev.CMP_EQ), consts
+
+
+def _device_program(prog):
+    """device predicates of a lowering.filter_program (connectives as PRED_AND / PRED_OR / PRED_NOT entries)"""
+    return [(_PRED_OPS[p], 0, dev.CMP_EQ, ()) if isinstance(p, str) else _device_pred(p) for p in prog]
+
+
+def _preds_fit(preds):
+    """a stage's device predicates are within the device's limits per call"""
+    ops = sum(p[0] in (dev.PRED_AND, dev.PRED_OR, dev.PRED_NOT) for p in preds)
+    return len(preds) - ops <= dev.PRED_MAX and ops <= dev.PRED_MAX_OPS and \
+        sum(len(p[3]) for p in preds) <= dev.PRED_MAX_CONSTS and \
+        sum(len(c.encode("utf-8")) for p in preds if p[0] == dev.PRED_STR for c in p[3]) <= dev.PRED_MAX_BYTES
 
 
 _FIELD_OP_NAMES = {dev.OP_SUM_I64: "sum_i64", dev.OP_MIN_I64: "min_i64", dev.OP_MAX_I64: "max_i64",
@@ -1345,7 +1375,7 @@ def _lower_map(runner, stage, inputs, si):
         runner.stats.add(stage, "device text tokenise+combine",
                          "bytes=%d terms=%d lines=%d" % (scan.nbytes, len(words), scan.n_lines))
         return f
-    m = _match_text_fields(stage, inputs)
+    m = _match_text_fields(stage, inputs, programs=True)
     if m is not None:
         if dist.active():
             raise NotLowerable("the field scan runs on one process")
@@ -1368,7 +1398,7 @@ def _lower_map(runner, stage, inputs, si):
             detail += " key=const" if len(expr[0][1]) == 1 and expr[0][1][0] & 0xFF == lowering.EV_CI else " key=expr"
         runner.stats.add(stage, "device text fields scan+combine", detail)
         return Frame(scan.keys, [scan.values], scalar=True, combined=True)
-    m = _match_json_fields(stage, inputs)
+    m = _match_json_fields(stage, inputs, programs=True)
     if m is not None:
         if dist.active():
             raise NotLowerable("the JSON field scan runs on one process")

@@ -206,7 +206,23 @@ int32_t dampr_table_fallback_lines(dampr_ctx *ctx, dampr_table *t, uint64_t *lin
 #define DAMPR_CMP_GE 5
 #define DAMPR_CMP_IN 6        /* STR and INT only: equal to one of the n constants                                */
 #define DAMPR_CMP_NOT_IN 7
-#define DAMPR_PRED_MAX 8              /* predicates per call                                                      */
+/* string tests and boolean structure: `"ERROR" in l`, `r[6].startswith("/api/")`, `len(l) > 90`, `l.strip()`,
+ * `r[1] == "GET" and (int(r[2]) >= 500 or not r[6].endswith(".js"))` */
+#define DAMPR_PRED_LEN 5      /* len() of a STR field (or the line) against one int64 (EQ .. GE)                    */
+#define DAMPR_PRED_NONBLANK 6 /* the STR field (or the line) holds a byte outside the str.split() whitespace class
+                                 (`x.strip()` as a truth value); cmp EQ, n = 0                                      */
+#define DAMPR_PRED_AND 7      /* connectives of a postfix program: pop b, pop a, push `a and b` / `a or b`; NOT    */
+#define DAMPR_PRED_OR 8       /* pops a and pushes `not a`. field, cmp and n are unused (n = 0)                    */
+#define DAMPR_PRED_NOT 9
+#define DAMPR_CMP_CONTAINS 8      /* STR only: the one constant is a substring of the field (`S in X`)            */
+#define DAMPR_CMP_NOT_CONTAINS 9  /* `S not in X`                                                                 */
+#define DAMPR_CMP_STARTS 10       /* STR only: the field starts with one of the n constants (`X.startswith(S)`)   */
+#define DAMPR_CMP_ENDS 11         /* `X.endswith(S)`                                                              */
+/* `field` of a STR, LEN or NONBLANK predicate that reads the whole line (no '\n'), not one of its fields: separator
+ * byte and DAMPR_FIELD_SEP_WS calls only */
+#define DAMPR_FIELD_LINE (-0x7FFFFFFF - 1)
+#define DAMPR_PRED_MAX_OPS 8          /* connectives per call                                                     */
+#define DAMPR_PRED_MAX 8              /* predicates (leaves) per call                                             */
 #define DAMPR_PRED_MAX_CONSTS 64      /* constants (set members included) over all predicates of a call           */
 #define DAMPR_PRED_MAX_BYTES 1024     /* bytes of STR constants over all predicates of a call                     */
 typedef struct dampr_field_pred {
@@ -230,7 +246,8 @@ typedef struct dampr_fields_spec {
                            DAMPR_OP_SUM_I64 (int() values) | DAMPR_OP_SUM_F64 (float() values)               */
     int32_t cr_is_data; /* 1: '\r' is an ordinary byte (binary-mode .gz); 0: it ends lines (text mode)        */
     const dampr_field_pred *preds; /* WHERE predicates, applied in order before the key and value are read       */
-    int32_t npreds;     /* 0 .. DAMPR_PRED_MAX; 0 (preds unused) is the plain scan                                */
+    int32_t npreds;     /* entries of preds: 0 .. DAMPR_PRED_MAX + DAMPR_PRED_MAX_OPS, at most DAMPR_PRED_MAX of
+                           them leaves and DAMPR_PRED_MAX_OPS connectives; 0 (preds unused) is the plain scan        */
 } dampr_fields_spec;
 /* WHERE (npreds > 0): on each line the device can take (the byte and length rules below), the predicates are
  * evaluated in order as Python's filters would be. The first false one drops the line: no key or value is read,
@@ -239,7 +256,16 @@ typedef struct dampr_fields_spec {
  * float() rule below) hands the line to the caller as a fallback line, whose filters then decide or raise. Only a
  * line that passes every predicate has its key and value read, under the rules below. A -0.0 in a predicate's field
  * does not set DAMPR_TF_NEGZERO. Dropped lines are counted: dampr_text_fields puts their number in stats[6];
- * in record mode it is stats[6] - stats[1] - stats[7] (records - folded lines - fallback lines). */
+ * in record mode it is stats[6] - stats[1] - stats[7] (records - folded lines - fallback lines).
+ * Programs: preds is a postfix program over leaves (every kind up to DAMPR_PRED_NONBLANK) and connectives. Each leaf
+ * is T, F or U (undecided: the cases above, a missing field or member, a JSON member that is not a string without
+ * escapes under CONTAINS .. ENDS, LEN or NONBLANK). Connectives combine left-sequentially, as Python's short circuit
+ * does: `a and b` is F if a is F, U if a is U, else b; `a or b` is T if a is T, U if a is U, else b; `not a` keeps U.
+ * The values left on the stack (one per filter call; a list without connectives leaves one per leaf, today's chain)
+ * are combined the same way with `and`, bottom first. F drops the line, U hands it to the caller, T reads the key and
+ * value. A program with a connective that finds fewer operands than it pops, more than DAMPR_PRED_MAX leaves or
+ * DAMPR_PRED_MAX_OPS connectives, a new kind or comparison under another kind than the ones named above, or (in a
+ * JSON call) DAMPR_FIELD_LINE returns DAMPR_ERR_ARG. */
 /* fold (key code -> value) of the lines whose first byte lies in [own_lo, own_hi) into the table (cleared by the
  * caller before the first range; ranges of one scan accumulate). Needs bytes [0, min(n, own_hi + DAMPR_FIELDS_HALO))
  * uploaded. The device folds a line only when every byte is ASCII and not NUL, it holds no '\r' (unless

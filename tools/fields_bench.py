@@ -6,7 +6,7 @@ from CUDA events (dampr_ctx_timings, DAMPR_K_TEXT_FIELDS) with its GB/s and shar
 page-cache-warm file, the host-map MB/s on a sample, and whether the device and the host results agree there.
 
     python tools/fields_bench.py [--gb 2] [--keys 1000000] [--reps 3] [--sample-mb 32] [--out DIR]
-                                 [--value int|float] [--op sum|min|max|mean] [--where none|str|int|float|set]
+                                 [--value int|float] [--op sum|min|max|mean] [--where none|str|int|float|set|contains|prefix|or|line]
                                  [--sep comma|ws] [--key-fields 1|2|3] [--expr none|product|ratio|nfields]
                                  [--key field|const|bucket]
 
@@ -23,6 +23,10 @@ MB/s, the stats line with filtered=N, and whether the host-map sample of the fil
   int    int(r[2]) >= 0           (the signed value field: about half; --value int only)
   float  float(r[2]) >= 0         (about half)
   set    r[0] not in <64 keys>    (keeps almost every line: each one is compared with all 64 members)
+  contains  'ab' in l             (a substring of the whole line, in front of the split: about one line in nine)
+  prefix    not r[1].startswith('x')                   (about 25 lines in 26)
+  or        r[0] < 'u0500000' or float(r[2]) >= 0      (about three quarters)
+  line      l.startswith('u0') and len(l) > 90         (every line at the default --keys, in front of the split)
 
 --sep ws writes the same rows with their fields joined by runs of 1-3 spaces or tabs instead of commas, a blank in
 front of about a quarter of them and behind another quarter (the filler field gives up the bytes, so every line keeps
@@ -176,7 +180,9 @@ def json_text(seed, n_lines, n_keys):
 
 SET_KEYS = tuple("u%07d" % (i * 7919) for i in range(64))
 WHERE = {"str": lambda r: r[0] < "u0500000", "int": lambda r: int(r[2]) >= 0, "float": lambda r: float(r[2]) >= 0,
-         "set": lambda r: r[0] not in SET_KEYS}
+         "set": lambda r: r[0] not in SET_KEYS, "prefix": lambda r: not r[1].startswith("x"),
+         "or": lambda r: r[0] < "u0500000" or float(r[2]) >= 0}
+LINE_WHERE = {"contains": lambda l: "ab" in l, "line": lambda l: l.startswith("u0") and len(l) > 90}   # on the line
 
 
 def rewrite_filler(text, seed, key_fields):
@@ -285,8 +291,11 @@ def job(Dampr, src, value="int", op="sum", where="none", sep="comma", key_fields
         return json_job(Dampr, src, value, op)
     conv = int if value == "int" else float
     key = KEY_FNS[key_fields]
-    d = Dampr.read_input(src).map(splitter(sep))
-    if where != "none":
+    d = Dampr.read_input(src)
+    if where in LINE_WHERE:
+        d = d.filter(LINE_WHERE[where])
+    d = d.map(splitter(sep))
+    if where in WHERE:
         d = d.filter(WHERE[where])
     if op == "mean":
         return d.mean(key, lambda r: conv(r[2]))
@@ -305,7 +314,8 @@ def python_fold(sample, value, op, where="none", sep="comma", key_fields=1):
     if sep == "json":
         rows = json_rows(sample, value)
     else:
-        rows = ((key(r), conv(r[2])) for r in map(split, sample.decode("ascii").split("\n")[:-1]) if keep(r))
+        lines = [l for l in sample.decode("ascii").split("\n")[:-1] if LINE_WHERE.get(where, lambda l: True)(l)]
+        rows = ((key(r), conv(r[2])) for r in map(split, lines) if keep(r))
     for k, v in rows:
         if op == "mean":
             s, n = out.get(k, (0, 0))
@@ -364,7 +374,8 @@ def main():
     ap.add_argument("--out", default=None, help="directory for the text file (default: a temporary one)")
     ap.add_argument("--value", choices=("int", "float"), default="int")
     ap.add_argument("--op", choices=("sum", "min", "max", "mean"), default="sum")
-    ap.add_argument("--where", choices=("none", "str", "int", "float", "set"), default="none")
+    ap.add_argument("--where", choices=("none", "str", "int", "float", "set", "contains", "prefix", "or", "line"),
+                    default="none")
     ap.add_argument("--sep", choices=("comma", "ws", ","), default="comma")
     ap.add_argument("--format", choices=("csv", "json"), default="csv")
     ap.add_argument("--key-fields", type=int, choices=(1, 2, 3), default=1)
