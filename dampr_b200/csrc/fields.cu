@@ -56,6 +56,15 @@
 // the line, so the representative is the line itself (offset << 20 | length, atomicMin keeps the lowest); an insert
 // that finds another line there splits that line again in global memory and compares the components (same_tuple).
 // table_tuple_keys_kernel decodes a tuple table the same way, from each entry's representative line.
+//
+// JSON paths (members r["a"]["b"].., their own builds, so the top-level JSON scans compile as before): the host
+// builds a trie of the wanted (parent, name) nodes. The line is validated by the same state machine, which also
+// tracks the node whose object it is in and compares names only there; a node's value clears the object bits and
+// member types of its subtree (the last occurrence of an interior name replaces its earlier subtree). A member whose
+// nodes above are not all objects at the line's end is one Python raises on: a read of it is a host line, a
+// predicate on it undecided.
+#include <type_traits>
+
 #include "common.cuh"
 #include "fparse.cuh"
 
@@ -537,6 +546,170 @@ __device__ __forceinline__ u32 member_bounds(const u32 (&mb)[JM], int j) {
     for (int i = 0; i < JM; ++i)
         if (i == j) b = mb[i];
     return b;
+}
+
+// ---- JSON paths: members r[n1]..[nk] ---------------------------------------------------------------------------
+constexpr int J_NODES = DAMPR_JSON_MAX_NODES;
+static_assert(J_NODES <= 16 && J_MAX <= 8, "node masks are u16, member type nibbles one u32");
+
+// the wanted paths of a JSON scan as a trie of (parent, name) nodes, passed by value in the kernel parameters
+struct JsonPathView {
+    u8 name[J_NODES][J_NAME];
+    u8 len[J_NODES];
+    signed char up[J_NODES];     // the parent node, -1 for a top-level name
+    signed char leaf[J_NODES];   // the member this node's value is, or -1
+    u16 kids[J_NODES + 1];       // kids[k + 1]: the nodes whose parent is k; kids[0]: the top-level names
+    u16 sub[J_NODES];            // the nodes beneath k
+    u32 sub_types[J_NODES];      // the type nibbles (of mt) of the members beneath k
+    u16 anc[J_MAX];              // the nodes above member j's own
+    signed char up_leaf[J_MAX];  // the member that is member j's parent node, or -1
+    int n;                       // members
+};
+
+// json_line over paths: the same validation, with names compared in the top-level object and in the object of each
+// interior node on a wanted path (an escaped name there returns false). A node's value replaces its earlier
+// occurrence's whole subtree. On return, member j's type is JT_NONE and bit j of bad is set when a node above it is
+// not an object in the line (missing, or its last occurrence is not an object): Python raises on reading it.
+template <int JM>
+__device__ __forceinline__ bool json_path_line(const u8 *t, u32 q, u32 end, const JsonPathView &jv, u32 (&mb)[JM],
+                                               u32 &mt, u32 &bad) {
+    enum { VALUE, VALUE_OR_CLOSE, NAME, NAME_OR_CLOSE, COLON, AFTER };
+    u64 objs = 0;     // bit d - 1: the container at depth d is an object
+    int depth = 0;
+    int st = VALUE;
+    int node = -1;    // the node whose object the scan compares names in (-1: the top-level object)
+    int nd = 1;       // that object's depth
+    int cur = -1;     // the child of node whose value comes next (depth nd)
+    u32 obj = 0;      // bit k: node k's last occurrence so far is an object
+    u32 p = q;
+    while (p < end) {
+        const u8 c = t[p];
+        if (c == ' ' || c == '\t' || c == '\r') {
+            ++p;
+            continue;
+        }
+        if ((st == NAME_OR_CLOSE || st == AFTER) && c == '}' && depth == nd && node >= 0) {
+            node = jv.up[node];   // leaving a wanted node's object (its '}' is checked below)
+            --nd;
+            cur = -1;
+        }
+        if (st == NAME_OR_CLOSE && c == '}') {
+            objs &= ~(1ULL << --depth);
+            st = AFTER;
+            ++p;
+            continue;
+        }
+        if (st == NAME_OR_CLOSE || st == NAME) {
+            u32 e;
+            bool esc;
+            if (c != '"' || !json_string(t, p, end, e, esc)) return false;
+            if (depth == nd) {
+                if (esc) return false;
+                const u32 len = e - p - 1;
+                cur = -1;
+                for (u32 km = jv.kids[node + 1]; km && cur < 0; km &= km - 1) {
+                    const int k = __ffs(km) - 1;
+                    if (len != jv.len[k]) continue;
+                    bool same = true;
+                    for (u32 i = 0; i < len && same; ++i) same = t[p + 1 + i] == jv.name[k][i];
+                    if (same) cur = k;
+                }
+            }
+            p = e + 1;
+            st = COLON;
+            continue;
+        }
+        if (st == COLON) {
+            if (c != ':') return false;
+            ++p;
+            st = VALUE;
+            continue;
+        }
+        if (st == AFTER) {
+            if (depth == 0) return false;
+            const bool ob = (objs >> (depth - 1)) & 1;
+            if (c == ',') st = ob ? NAME : VALUE;
+            else if (c == (ob ? '}' : ']')) objs &= ~(1ULL << --depth);
+            else return false;
+            ++p;
+            continue;
+        }
+        if (st == VALUE_OR_CLOSE && c == ']') {
+            --depth;
+            st = AFTER;
+            ++p;
+            continue;
+        }
+        if (depth == 0 && c != '{') return false;
+        const int k = depth == nd ? cur : -1;   // the wanted node this value belongs to
+        if (k >= 0) {   // a new occurrence: forget the earlier one's subtree
+            obj = (obj & ~(u32)jv.sub[k] & ~(1u << k)) | (u32)(c == '{') << k;
+            mt &= ~jv.sub_types[k];
+        }
+        u32 vs = p;
+        int ty = JT_OTHER;
+        st = AFTER;
+        if (c == '{' || c == '[') {
+            if (depth == J_DEPTH) return false;
+            if (c == '{') objs |= 1ULL << depth;
+            ++depth;
+            st = c == '{' ? NAME_OR_CLOSE : VALUE_OR_CLOSE;
+            ++p;
+            if (k >= 0 && c == '{' && jv.kids[k + 1]) {   // descend into a wanted interior node
+                node = k;
+                nd = depth;
+                cur = -1;
+            }
+        } else if (c == '"') {
+            u32 e;
+            bool esc;
+            if (!json_string(t, p, end, e, esc)) return false;
+            ty = esc ? JT_ESC : JT_STR;
+            vs = p + 1;
+            p = e;
+        } else if (c == '-' || is_digit(c)) {
+            u32 i = p + (c == '-');
+            if (t[i] == '0') ++i;
+            else if (is_digit(t[i])) i = skip_digits(t, i + 1);
+            else return false;
+            ty = JT_INT;
+            if (t[i] == '.') {
+                if (!is_digit(t[i + 1])) return false;
+                i = skip_digits(t, i + 2);
+                ty = JT_FLOAT;
+            }
+            if ((t[i] | 0x20) == 'e') {
+                ++i;
+                if (t[i] == '+' || t[i] == '-') ++i;
+                if (!is_digit(t[i])) return false;
+                i = skip_digits(t, i + 1);
+                ty = JT_FLOAT;
+            }
+            p = i;
+        } else {
+            const u32 n = c == 'f' ? 5u : 4u;
+            if (!lit_at(t, p, end, c == 't' ? "true" : c == 'f' ? "false" : "null", n)) return false;
+            p += n;
+        }
+        if (k >= 0) {
+            const int lf = jv.leaf[k];
+#pragma unroll
+            for (int j = 0; j < JM; ++j)
+                if (j == lf) {
+                    mb[j] = vs | p << 16;
+                    mt = (mt & ~(0xFu << (4 * j))) | (u32)ty << (4 * j);
+                }
+        }
+        if (ty == JT_STR || ty == JT_ESC) ++p;
+    }
+    if (st != AFTER || depth != 0) return false;
+#pragma unroll
+    for (int j = 0; j < JM; ++j)
+        if (j < jv.n && (jv.anc[j] & ~obj)) {
+            bad |= 1u << j;
+            mt &= ~(0xFu << (4 * j));
+        }
+    return true;
 }
 
 __device__ __forceinline__ u64 hash_bytes(const u8 *p, u32 len, u64 seed) {
@@ -1024,17 +1197,22 @@ __global__ void __launch_bounds__(SCAN_THREADS) fields_tile_scan_kernel(u64 *til
 // a JSON scan's work on one line after pass 1 (t[q, end) is ASCII and ends at its '\n'): validate it, evaluate the
 // predicates on its members, then read the key and the value. Sets to_host, dropped, val, code and rep as the field
 // path does (g0: the global offset of window position 0). A kept line's key and value kinds are both reported before
-// either decides that the line is the host's.
-template <int VK, bool WHERE>
+// either decides that the line is the host's. JV: JsonView (top-level members) or JsonPathView (paths).
+template <int VK, bool WHERE, class JV>
 __device__ __forceinline__ void json_fold(const u8 *t, u32 q, u32 end, u64 g0, const FieldsView &tab,
-                                          const JsonView &jv, const WhereView *where, bool &to_host, bool &dropped,
+                                          const JV &jv, const WhereView *where, bool &to_host, bool &dropped,
                                           long long &val, u64 &code, u64 &rep, u64 &acc_long, u32 &flags) {
+    constexpr bool PATHS = std::is_same<JV, JsonPathView>::value;
     constexpr int JM = WHERE ? J_MAX : 2;   // the plain scan reads the key and the value only
     u32 mb[JM];
 #pragma unroll
     for (int j = 0; j < JM; ++j) mb[j] = 0;
     u32 mt = 0;
-    if (!json_line<JM>(t, q, end, jv, mb, mt)) {
+    u32 bad = 0;   // PATHS: the members with a missing or non-object node above them
+    bool valid;
+    if constexpr (PATHS) valid = json_path_line<JM>(t, q, end, jv, mb, mt, bad);
+    else valid = json_line<JM>(t, q, end, jv, mb, mt);
+    if (!valid) {
         to_host = true;
         return;
     }
@@ -1051,6 +1229,18 @@ __device__ __forceinline__ void json_fold(const u8 *t, u32 q, u32 end, u64 g0, c
                 int r;
                 if (pr.kind == DAMPR_PRED_MEMBER) {
                     r = (ty != JT_NONE) == (pr.cmp == DAMPR_CMP_IN);
+                    if constexpr (PATHS) {
+                        if ((bad >> pr.field) & 1u) {   // "m" in x where x is not a present object
+                            r = -1;
+                            const int pl = jv.up_leaf[pr.field];
+                            if (pr.n == 1 && pl >= 0 && ((mt >> (4 * pl)) & 0xFu) == JT_STR) {   // x is a str
+                                const u32 b = member_bounds<JM>(mb, pl);
+                                const long long k = wh.c[pr.first];
+                                r = contains(t + (b & 0xFFFFu), (b >> 16) - (b & 0xFFFFu), wh.b + (k >> 32), (u32)k) ==
+                                    (pr.cmp == DAMPR_CMP_IN);
+                            }
+                        }
+                    }
                 } else {
                     // a member of another type than the constant's, or a missing one: the host's filter decides
                     const bool has = pr.kind == DAMPR_PRED_INT ? ty == JT_INT
@@ -1121,11 +1311,13 @@ __device__ __forceinline__ void json_fold(const u8 *t, u32 q, u32 end, u64 g0, c
 // whitespace (`line.split()`) instead of the separator byte; JSON: json.loads each line and read the members *json;
 // TUP: the key is the tuple of the components that follow the predicates (where points into a TupleWhere;
 // tab.key_field is component 0's field, tab.key_int is not read); EXPR: the load slots follow the predicates as TUP's
-// components do, and the programs follow them (where points into an ExprWhere)
-template <int VK, int MODE, bool WHERE, bool WS, bool JSON = false, bool TUP = false, bool EXPR = false>
+// components do, and the programs follow them (where points into an ExprWhere); JV: JsonPathView for a JSON scan
+// over paths
+template <int VK, int MODE, bool WHERE, bool WS, bool JSON = false, bool TUP = false, bool EXPR = false,
+          class JV = JsonView>
 __device__ __forceinline__ void fields_tiles(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi,
                                              const FieldsView &tab, const RecView &rv, const WhereView *where,
-                                             const JsonView *json = nullptr) {
+                                             const JV *json = nullptr) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SmemF &s = *reinterpret_cast<SmemF *>(smem_raw);
     const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1613,6 +1805,24 @@ text_json_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_
 }
 static_assert(sizeof(Where) + sizeof(JsonView) + 256 <= 4096, "kernel parameters");
 
+// the JSON-lines builds over paths: the trie (and a WHERE scan's predicates) read in place from the parameters
+template <int VK, int MODE>
+__global__ void __launch_bounds__(F_THREADS, 4)
+text_json_path_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv,
+                             const __grid_constant__ JsonPathView json) {
+    fields_tiles<VK, MODE, false, false, true, false, false, JsonPathView>(text, n, own_lo, own_hi, tab, rv, nullptr,
+                                                                           &json);
+}
+
+template <int VK, int MODE>
+__global__ void __launch_bounds__(F_THREADS, 4)
+text_json_path_fields_kernel(const u8 *__restrict__ text, u64 n, u64 own_lo, u64 own_hi, FieldsView tab, RecView rv,
+                             const __grid_constant__ JsonPathView json, const __grid_constant__ Where where) {
+    fields_tiles<VK, MODE, true, false, true, false, false, JsonPathView>(text, n, own_lo, own_hi, tab, rv, &where.v,
+                                                                          &json);
+}
+static_assert(sizeof(Where) + sizeof(JsonPathView) + 256 <= 4096, "kernel parameters");
+
 // the tuple-key builds (plain and WHERE) of the separator-byte and whitespace scans: the components (and the
 // predicates, unused by a plain build) read in place from the parameters. As for the JSON builds, saying that the
 // plain builds run 4 CTAs per SM keeps ptxas from squeezing them into 40 registers and spilling.
@@ -1638,11 +1848,11 @@ static_assert(sizeof(ExprWhere) + 256 <= 4096, "kernel parameters");
 
 // one kernel over the tiles of [own_lo, own_hi); WHERE: the build that applies the predicates *wh; WS: the
 // whitespace-split build; JSON: the JSON-lines build over the members *jv; TUP: the tuple-key build over *tk; xe: the
-// expression build over the load slots *tk and the programs *xe
+// expression build over the load slots *tk and the programs *xe; pv: the JSON build over the member paths *pv
 template <int VK, int MODE, bool WHERE = false, bool WS = false, bool JSON = false, bool TUP = false>
 int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const FieldsView &tv, const RecView &rv,
                   int timer, const Where *wh = nullptr, const JsonView *jv = nullptr,
-                  const TupleView *tk = nullptr, const ExprView *xe = nullptr) {
+                  const TupleView *tk = nullptr, const ExprView *xe = nullptr, const JsonPathView *pv = nullptr) {
     const size_t smem = sizeof(SmemF);
     const u64 ntiles = (own_hi - own_lo + F_OWN - 1) / F_OWN;
     u64 grid = (u64)ctx->num_sms * 4;
@@ -1675,16 +1885,32 @@ int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, con
         ScopedTimer tm(ctx, timer);
         kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, tw);
     } else if constexpr (JSON && WHERE) {
-        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonView, Where) =
-            text_json_fields_kernel<VK, MODE>;
-        CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ScopedTimer tm(ctx, timer);
-        kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *jv, *wh);
+        if (pv) {
+            void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonPathView, Where) =
+                text_json_path_fields_kernel<VK, MODE>;
+            CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            ScopedTimer tm(ctx, timer);
+            kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *pv, *wh);
+        } else {
+            void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonView, Where) =
+                text_json_fields_kernel<VK, MODE>;
+            CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            ScopedTimer tm(ctx, timer);
+            kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *jv, *wh);
+        }
     } else if constexpr (JSON) {
-        void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonView) = text_json_fields_kernel<VK, MODE>;
-        CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ScopedTimer tm(ctx, timer);
-        kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *jv);
+        if (pv) {
+            void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonPathView) =
+                text_json_path_fields_kernel<VK, MODE>;
+            CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            ScopedTimer tm(ctx, timer);
+            kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *pv);
+        } else {
+            void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, JsonView) = text_json_fields_kernel<VK, MODE>;
+            CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            ScopedTimer tm(ctx, timer);
+            kernel<<<(unsigned)grid, F_THREADS, smem, ctx->stream>>>(tb->text, tb->n, own_lo, own_hi, tv, rv, *jv);
+        }
     } else if constexpr (WHERE) {
         void (*kernel)(const u8 *, u64, u64, u64, FieldsView, RecView, Where) =
             text_fields_kernel<VK, MODE, true, WS>;
@@ -1702,8 +1928,10 @@ int launch_fields(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, con
 }
 
 // the predicates of spec in kernel-parameter form; DAMPR_ERR_ARG for a kind, comparison or limit outside the header's
-// (json: the predicates of a JSON scan, whose fields index the nmembers members; DAMPR_PRED_MEMBER instead of NFIELDS)
-int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, Where &wv, bool json = false, int nmembers = 0) {
+// (json: the predicates of a JSON scan, whose fields index the nmembers members; DAMPR_PRED_MEMBER instead of NFIELDS;
+// paths: a call over member paths, whose DAMPR_PRED_MEMBER may carry one STR constant)
+int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, Where &wv, bool json = false, int nmembers = 0,
+               bool paths = false) {
     ARG_CHECK(ctx, spec->npreds >= 0 && spec->npreds <= DAMPR_PRED_MAX + DAMPR_PRED_MAX_OPS,
               "npreds must be 0 .. DAMPR_PRED_MAX + DAMPR_PRED_MAX_OPS");
     ARG_CHECK(ctx, spec->npreds == 0 || spec->preds != nullptr, "null preds");
@@ -1748,7 +1976,8 @@ int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, Where &wv, bool js
         ARG_CHECK(ctx, p.cmp < DAMPR_CMP_CONTAINS || p.kind == DAMPR_PRED_STR, "CONTAINS .. ENDS take STR");
         ARG_CHECK(ctx, p.kind != DAMPR_PRED_LEN || p.cmp <= DAMPR_CMP_GE, "LEN takes EQ .. GE");
         ARG_CHECK(ctx, p.kind != DAMPR_PRED_NONBLANK || p.cmp == DAMPR_CMP_EQ, "NONBLANK takes EQ");
-        ARG_CHECK(ctx, member || p.kind == DAMPR_PRED_NONBLANK ? p.n == 0
+        ARG_CHECK(ctx, member                               ? (p.n == 0 || (paths && p.n == 1))
+                       : p.kind == DAMPR_PRED_NONBLANK      ? p.n == 0
                        : in || any                          ? (p.n >= 1 && p.n <= DAMPR_PRED_MAX_CONSTS)
                                                             : p.n == 1,
                   "predicate constant count");
@@ -1759,7 +1988,7 @@ int where_view(dampr_ctx *ctx, const dampr_fields_spec *spec, Where &wv, bool js
                 long long bits;
                 memcpy(&bits, &p.f64, sizeof bits);
                 w.c[nc] = bits;
-            } else if (p.kind == DAMPR_PRED_STR) {
+            } else if (p.kind == DAMPR_PRED_STR || member) {
                 ARG_CHECK(ctx, p.bytes != nullptr && p.lens != nullptr, "null predicate strings");
                 ARG_CHECK(ctx, p.lens[i] <= (uint32_t)(DAMPR_PRED_MAX_BYTES - nb),
                           "more than DAMPR_PRED_MAX_BYTES bytes of predicate strings");
@@ -1791,9 +2020,73 @@ int check_fields_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own
     return where_view(ctx, spec, w);
 }
 
-// the arguments of a JSON call and its member names in kernel-parameter form
+// the trie of a JSON call whose members hold a path (names joined by DAMPR_JSON_PATH_SEP)
+int json_path_view(dampr_ctx *ctx, const dampr_json_members *m, JsonPathView &pv) {
+    pv = JsonPathView{};
+    pv.n = m->n;
+    for (int k = 0; k < J_NODES; ++k) pv.up[k] = pv.leaf[k] = -1;
+    int nn = 0, off = 0;
+    int node_of[J_MAX];
+    for (int j = 0; j < m->n; ++j) {
+        const int len = m->len[j];
+        ARG_CHECK(ctx, len >= 0 && len < DAMPR_JSON_MAX_PATH * (J_NAME + 1),
+                  "a member of 1 .. DAMPR_JSON_MAX_PATH names of 0 .. DAMPR_JSON_MAX_NAME bytes");
+        const char *b = m->bytes + off;
+        int names = 1;
+        for (int i = 0; i < len; ++i) names += b[i] == DAMPR_JSON_PATH_SEP;
+        ARG_CHECK(ctx, names <= DAMPR_JSON_MAX_PATH, "a path of more than DAMPR_JSON_MAX_PATH names");
+        int parent = -1, s = 0;
+        u16 anc = 0;
+        for (int x = 0; x < names; ++x) {
+            int e = s;
+            while (e < len && b[e] != DAMPR_JSON_PATH_SEP) ++e;
+            const int nl = e - s;
+            ARG_CHECK(ctx, names == 1 || nl >= 1, "an empty name in a path");
+            ARG_CHECK(ctx, nl <= J_NAME, "a member name of 0 .. DAMPR_JSON_MAX_NAME bytes");
+            for (int i = s; i < e; ++i) {
+                const u8 c = (u8)b[i];
+                ARG_CHECK(ctx, c >= 0x20 && c < 0x80 && c != '"' && c != '\\',
+                          "member names are ASCII without '\"', '\\\\' or bytes below 0x20");
+            }
+            int k = 0;
+            while (k < nn && !(pv.up[k] == parent && pv.len[k] == nl && memcmp(pv.name[k], b + s, nl) == 0)) ++k;
+            if (k == nn) {
+                ARG_CHECK(ctx, nn < J_NODES, "more than DAMPR_JSON_MAX_NODES path nodes");
+                pv.up[k] = (signed char)parent;
+                pv.len[k] = (u8)nl;
+                memcpy(pv.name[k], b + s, nl);
+                ++nn;
+            }
+            if (x + 1 < names) {
+                anc |= (u16)(1u << k);
+                parent = k;
+            } else {
+                ARG_CHECK(ctx, pv.leaf[k] < 0, "two members name the same path");
+                pv.leaf[k] = (signed char)j;
+                pv.anc[j] = anc;
+                node_of[j] = k;
+            }
+            s = e + 1;
+        }
+        off += len;
+    }
+    for (int j = 0; j < m->n; ++j)
+        pv.up_leaf[j] = pv.up[node_of[j]] >= 0 ? pv.leaf[pv.up[node_of[j]]] : (signed char)-1;
+    for (int k = 0; k < nn; ++k) {
+        pv.kids[pv.up[k] + 1] |= (u16)(1u << k);
+        for (int a = pv.up[k]; a >= 0; a = pv.up[a]) {
+            pv.sub[a] |= (u16)(1u << k);
+            if (pv.leaf[k] >= 0) pv.sub_types[a] |= 0xFu << (4 * pv.leaf[k]);
+        }
+    }
+    return DAMPR_OK;
+}
+
+// the arguments of a JSON call in kernel-parameter form: its predicates w, and its members as the names jv, or as the
+// trie pv (paths set) when a member is a path
 int check_json_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own_lo, u64 own_hi,
-                    const dampr_fields_spec *spec, const dampr_json_members *m, JsonView &jv) {
+                    const dampr_fields_spec *spec, const dampr_json_members *m, JsonView &jv, JsonPathView &pv,
+                    bool &paths, Where &w) {
     ARG_CHECK(ctx, ctx && t && tb && spec && m, "null");
     ARG_CHECK(ctx, own_lo <= own_hi && own_hi <= tb->n, "ownership range outside the text");
     ARG_CHECK(ctx, (own_lo % 16) == 0, "own_lo must be a multiple of 16");
@@ -1804,6 +2097,15 @@ int check_json_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own_l
     ARG_CHECK(ctx, spec->key_field >= 0 && spec->key_field < m->n, "key_field must index the members");
     ARG_CHECK(ctx, spec->val_field == DAMPR_FIELD_VAL_ONE || (spec->val_field >= 0 && spec->val_field < m->n),
               "val_field must index the members or be DAMPR_FIELD_VAL_ONE");
+    paths = false;
+    for (int j = 0, off = 0; j < m->n && m->len[j] >= 0 && m->len[j] < DAMPR_JSON_MAX_PATH * (J_NAME + 1); ++j) {
+        paths |= memchr(m->bytes + off, DAMPR_JSON_PATH_SEP, m->len[j]) != nullptr;
+        off += m->len[j];
+    }
+    if (paths) {
+        if (int r = json_path_view(ctx, m, pv)) return r;
+        return where_view(ctx, spec, w, true, m->n, true);
+    }
     jv = JsonView{};
     jv.n = m->n;
     int off = 0;
@@ -1818,7 +2120,6 @@ int check_json_args(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, u64 own_l
         jv.len[j] = (u8)m->len[j];
         off += m->len[j];
     }
-    Where w;
     return where_view(ctx, spec, w, true, m->n);
 }
 
@@ -1854,17 +2155,17 @@ int launch_fold_sep(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, c
                                                           nullptr, tk);
 }
 
-// the fold pass of one range of a JSON scan: the plain build reads two members, the WHERE build (also taken without
-// predicates when more members are listed) up to J_MAX
+// the fold pass of one range of a JSON scan over the names jv, or the member paths *pv: the plain build reads two
+// members, the WHERE build (also taken without predicates when more members are listed) up to J_MAX
 template <int VK, int MODE>
 int launch_json_fold(dampr_ctx *ctx, dampr_textbuf *tb, u64 own_lo, u64 own_hi, const dampr_fields_spec *spec,
-                     const JsonView &jv, const FieldsView &tv, const RecView &rv) {
-    if (spec->npreds == 0 && jv.n <= 2)
+                     const JsonView &jv, const JsonPathView *pv, const Where &w, const FieldsView &tv,
+                     const RecView &rv) {
+    if (spec->npreds == 0 && (pv ? pv->n : jv.n) <= 2)
         return launch_fields<VK, MODE, false, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS,
-                                                          nullptr, &jv);
-    Where w;
-    if (int r = where_view(ctx, spec, w, true, jv.n)) return r;
-    return launch_fields<VK, MODE, true, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w, &jv);
+                                                          nullptr, &jv, nullptr, nullptr, pv);
+    return launch_fields<VK, MODE, true, false, true>(ctx, tb, own_lo, own_hi, tv, rv, DAMPR_K_TEXT_FIELDS, &w, &jv,
+                                                      nullptr, nullptr, pv);
 }
 
 // the fold pass of one range: the separator-byte build, or the whitespace-split one under DAMPR_FIELD_SEP_WS
@@ -2088,7 +2389,11 @@ extern "C" int32_t dampr_text_json_fields(dampr_ctx *ctx, dampr_table *t, dampr_
                                           uint64_t own_hi, const dampr_fields_spec *spec,
                                           const dampr_json_members *members) {
     JsonView jv;
-    if (int r = check_json_args(ctx, t, tb, own_lo, own_hi, spec, members, jv)) return r;
+    JsonPathView pv;
+    bool paths;
+    Where w;
+    if (int r = check_json_args(ctx, t, tb, own_lo, own_hi, spec, members, jv, pv, paths, w)) return r;
+    const JsonPathView *p = paths ? &pv : nullptr;
     const bool f64 = spec->op == DAMPR_OP_MIN_F64 || spec->op == DAMPR_OP_MAX_F64;
     ARG_CHECK(ctx, f64 || spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_MIN_I64 ||
                        spec->op == DAMPR_OP_MAX_I64,
@@ -2097,15 +2402,19 @@ extern "C" int32_t dampr_text_json_fields(dampr_ctx *ctx, dampr_table *t, dampr_
     if (own_hi <= own_lo) return DAMPR_OK;
     const FieldsView tv = fields_view(t, spec, spec->op);
     wait_uploads(ctx);
-    if (f64) return launch_json_fold<VK_F64, M_TABLE>(ctx, tb, own_lo, own_hi, spec, jv, tv, RecView{});
-    return launch_json_fold<VK_INT, M_TABLE>(ctx, tb, own_lo, own_hi, spec, jv, tv, RecView{});
+    if (f64) return launch_json_fold<VK_F64, M_TABLE>(ctx, tb, own_lo, own_hi, spec, jv, p, w, tv, RecView{});
+    return launch_json_fold<VK_INT, M_TABLE>(ctx, tb, own_lo, own_hi, spec, jv, p, w, tv, RecView{});
 }
 
 extern "C" int32_t dampr_text_json_fields_records(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb,
                                                   uint64_t own_lo, uint64_t own_hi, const dampr_fields_spec *spec,
                                                   const dampr_json_members *members, dampr_kv *rec) {
     JsonView jv;
-    if (int r = check_json_args(ctx, t, tb, own_lo, own_hi, spec, members, jv)) return r;
+    JsonPathView pv;
+    bool paths;
+    Where w;
+    if (int r = check_json_args(ctx, t, tb, own_lo, own_hi, spec, members, jv, pv, paths, w)) return r;
+    const JsonPathView *p = paths ? &pv : nullptr;
     ARG_CHECK(ctx, rec != nullptr, "null");
     ARG_CHECK(ctx, spec->op == DAMPR_OP_SUM_I64 || spec->op == DAMPR_OP_SUM_F64,
               "op must be DAMPR_OP_SUM_I64 or DAMPR_OP_SUM_F64");
@@ -2115,8 +2424,8 @@ extern "C" int32_t dampr_text_json_fields_records(dampr_ctx *ctx, dampr_table *t
     RecView rv{rec->rec, rec->capacity, nullptr};
     if (int r = count_records(ctx, t, tb, own_lo, own_hi, tv, rv)) return r;
     if (spec->op == DAMPR_OP_SUM_F64)
-        return launch_json_fold<VK_F64, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, jv, tv, rv);
-    return launch_json_fold<VK_INT, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, jv, tv, rv);
+        return launch_json_fold<VK_F64, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, jv, p, w, tv, rv);
+    return launch_json_fold<VK_INT, M_RECORDS>(ctx, tb, own_lo, own_hi, spec, jv, p, w, tv, rv);
 }
 
 extern "C" int32_t dampr_text_fields_tuple(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo,

@@ -36,6 +36,7 @@ FIELD_VAL_ONE = 0x7FFFFFFF
 FIELD_SEP_WS = 256   # sep: split like str.split() (runs of ASCII whitespace, no '' fields)
 FIELD_SEP_JSON = 257   # sep of the JSON-lines calls: fields are the members of json.loads(line)
 JSON_MAX_MEMBERS, JSON_MAX_NAME, JSON_MAX_DEPTH = 8, 64, 64
+JSON_PATH_SEP, JSON_MAX_PATH, JSON_MAX_NODES = 0x1F, 4, 16   # member paths: names joined by JSON_PATH_SEP
 FIELDS_HALO = 65536
 FIELD_KEYS_MAX = 4   # components of a tuple key (dampr_field_keys)
 # computed keys and values of a field scan (dampr_field_expr): limits, program types, load slot kinds
@@ -86,7 +87,8 @@ class FieldsSpec(C.Structure):
 def fields_spec(spec, cr_is_data, preds):
     """dampr_fields_spec of spec = (sep byte or FIELD_SEP_WS, key field, key kind, value field or FIELD_VAL_ONE, op)
     and the WHERE predicates preds = [(PRED_*, field, CMP_*, constants)]: constants a tuple of str (PRED_STR), int
-    (PRED_INT, PRED_NFIELDS, PRED_LEN) or one float (PRED_F64), () for PRED_NONBLANK, PRED_MEMBER and the connectives
+    (PRED_INT, PRED_NFIELDS, PRED_LEN) or one float (PRED_F64), () for PRED_NONBLANK, PRED_MEMBER (or, over member
+    paths, the member's last name, a str) and the connectives
     PRED_AND / PRED_OR / PRED_NOT of a postfix program. The returned structure keeps its constant arrays alive."""
     sep, kf, kind, vf, op = spec
     arr = (FieldPred * max(1, len(preds)))()
@@ -95,7 +97,7 @@ def fields_spec(spec, cr_is_data, preds):
         p.kind, p.field, p.cmp, p.n = int(pk), int(field), int(cmp), len(consts)
         if pk == PRED_F64:
             p.f64 = float(consts[0])
-        elif pk == PRED_STR:
+        elif pk == PRED_STR or pk == PRED_MEMBER:   # a member test's one constant: the substring of a str container
             raw = [c.encode("utf-8") for c in consts]
             b = (C.c_uint8 * max(1, sum(map(len, raw)))).from_buffer_copy(b"".join(raw).ljust(1, b"\0"))
             ln = (C.c_uint32 * len(raw))(*map(len, raw))
@@ -161,8 +163,10 @@ class JsonMembers(C.Structure):
 
 
 def json_members(names):
-    """dampr_json_members of the member names (str); the returned structure keeps its arrays alive"""
-    raw = [n.encode("ascii") for n in names]
+    """dampr_json_members of the members: a name (str) or a path (a tuple of names, joined by JSON_PATH_SEP); the
+    returned structure keeps its arrays alive"""
+    raw = [bytes([JSON_PATH_SEP]).join(x.encode("ascii") for x in n) if isinstance(n, tuple) else n.encode("ascii")
+           for n in names]
     ln = (C.c_int32 * max(1, len(raw)))(*map(len, raw))
     m = JsonMembers(len(raw), b"".join(raw), C.cast(ln, C.POINTER(C.c_int32)))
     m._keep = ln

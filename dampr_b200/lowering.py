@@ -503,6 +503,29 @@ def _member(e):
     return (kind, name) if ok and json_member_name(name) else None
 
 
+JSON_MAX_PATH = 4   # names per member path (DAMPR_JSON_MAX_PATH)
+
+
+def _path(e):
+    """(kind, path) if e is r[n1]..[nk] (FIELD_DATA), int() (FIELD_INT) or float() (FIELD_FLOAT) of it over the
+    argument r, path the tuple of 1 .. JSON_MAX_PATH constant names the device matches (none empty in a path of two or
+    more: the device cannot name them), else None. Array indices (r["a"][0]) and r.get are None."""
+    kind = FIELD_DATA
+    if isinstance(e, E) and e.op == "call" and isinstance(e.a, E) and e.a.op == "obj" and e.a.a in (int, float) \
+            and len(e.b) == 1:
+        kind, e = FIELD_INT if e.a.a is int else FIELD_FLOAT, e.b[0]
+    names = []
+    while isinstance(e, E) and e.op == "sub" and len(names) <= JSON_MAX_PATH:
+        ok, name = _const(e.b)
+        if not ok or not json_member_name(name):
+            return None
+        names.append(name)
+        e = e.a
+    if not _is_arg(e) or not 1 <= len(names) <= JSON_MAX_PATH or (len(names) > 1 and not all(names)):
+        return None
+    return kind, tuple(reversed(names))
+
+
 def json_fields_spec(key_fn, value_fn):
     """Device JSON-lines spec of a keyed(key_fn, value_fn) behind map(json.loads): (key name, key kind, value name,
     value kind, mean) where the key is r["k"] (FIELD_DATA) or int(r["k"]) (FIELD_INT), and the value is
@@ -510,13 +533,28 @@ def json_fields_spec(key_fn, value_fn):
       r["v"] (FIELD_DATA), int(r["v"]) or float(r["v"])     mean False
       mean()'s `(value(r), 1)`, value one of those          mean True
     None for any other shape (r.get, r["a"]["b"], tuple keys, float keys, ...)."""
+    return _json_spec(key_fn, value_fn, _member)
+
+
+def json_fields_path_spec(key_fn, value_fn):
+    """json_fields_spec over member paths: the key r[n1]..[nk] or int() of it, the value 1, r[n1]..[nk], int() or
+    float() of it (or mean()'s pair), 1 <= k <= JSON_MAX_PATH, each name a tuple of names. None unless the key or the
+    value is a path of two or more names (json_fields_spec takes the rest)."""
+    spec = _json_spec(key_fn, value_fn, _path)
+    if spec is None or not any(p is not None and len(p) > 1 for p in (spec[0], spec[2])):
+        return None
+    return spec
+
+
+def _json_spec(key_fn, value_fn, member):
+    """json_fields_spec's result with member(e) reading the key's and the value's members"""
     fns = (key_fn, value_fn)
     if not all(isinstance(f, types.FunctionType) and f.__code__.co_argcount == 1 for f in fns):
         return None
     ke, ve = analyze(key_fn), analyze(value_fn)
     if ke is None or ve is None:
         return None
-    k = _member(ke)
+    k = member(ke)
     if k is None or k[0] == FIELD_FLOAT:
         return None
     if _is_one(ve):
@@ -527,7 +565,7 @@ def json_fields_spec(key_fn, value_fn):
         if inner is None or not _is_one(ve.a[1]):
             return None
         ve = inner
-    v = _member(ve)
+    v = member(ve)
     if v is None:
         return None
     return k[1], k[0], v[1], v[0], mean
@@ -550,16 +588,24 @@ def json_predicate(fn):
     return _json_leaf(e)
 
 
-def _json_leaf(e):
-    """json_predicate's result for the comparison tree e"""
+def _json_leaf(e, paths=False):
+    """json_predicate's result for the comparison tree e; with `paths` the members are _path's paths, and
+    "m" in r[n1]..[nk] (1 <= k < JSON_MAX_PATH) is (FIELD_MEMBER, (n1, .., nk, m), op, ("m",)): Python's `in` on
+    whatever r[n1]..[nk] is, membership where it is an object and the substring test where it is a str"""
     op, l, r = e.a, e.b, e.c
     if op in ("in", "not in") and _is_arg(r):
         ok, name = _const(l)
         return (FIELD_MEMBER, name, op, ()) if ok and json_member_name(name) else None
+    if paths and op in ("in", "not in"):
+        under = _path(r)
+        if under is not None and under[0] == FIELD_DATA:
+            ok, name = _const(l)
+            m = _path(E("sub", r, E("const", name))) if ok else None
+            return None if m is None else (FIELD_MEMBER, m[1], op, (name,))
     if op in _FLIP and _pred_const(l)[0] and not _pred_const(r)[0]:
         op, l, r = _FLIP[op], r, l
     ok, c = _pred_const(r)
-    m = _member(l)
+    m = _path(l) if paths else _member(l)
     if not ok or m is None:
         return None
     kind, name = m
@@ -762,23 +808,55 @@ def json_filter_program(fn):
     e = analyze(fn)
     if e is None:
         return None
+    return _program(e, _json_program_leaf)
 
-    def operand(x):
-        m = _member(x)
-        return m[1] if m is not None and m[0] == FIELD_DATA else None
+
+def json_path_filter_program(fn):
+    """The program of a filter in a stage that reads member paths: json_filter_program over paths r[n1]..[nk]
+    (1 <= k <= JSON_MAX_PATH, each name a tuple of names), its leaves and string tests on paths, and
+    "m" in r[n1]..[nk] / "m" not in r[n1]..[nk] for k >= 1 as _json_leaf gives them (the path (n1, .., nk, m) with the
+    constant ("m",): the device decides membership where r[n1]..[nk] is an object, the substring test where it is a
+    str without escapes). A name the device cannot match keeps json_filter_program's substring leaf on r["a"] and is
+    refused deeper. None unless some leaf reads a path of two or more names."""
+    if not (isinstance(fn, types.FunctionType) and fn.__code__.co_argcount == 1):
+        return None
+    e = analyze(fn)
+    if e is None:
+        return None
 
     def leaf(x):
         if x.op == "cmp":
-            p = _json_leaf(x)
+            p = _json_leaf(x, paths=True)
             if p is not None:
-                return p
-        got = _str_leaf(x, operand)
-        if got is None:
-            return None
-        op, kind, name, consts = got
-        return kind, name, op, consts
+                kind, name, op, consts = p
+                return kind, name if isinstance(name, tuple) else (name,), op, consts
+        p = _json_program_leaf(x)
+        if p is not None:
+            kind, name, op, consts = p
+            return kind, (name,), op, consts
+        return _json_program_leaf(x, paths=True)
 
-    return _program(e, leaf)
+    prog = _program(e, leaf)
+    if prog is None or not any(not isinstance(x, str) and len(x[1]) > 1 for x in prog):
+        return None
+    return prog
+
+
+def _json_program_leaf(x, paths=False):
+    """a leaf of json_filter_program (kind, name, op, constants), or None; with `paths` over _path's paths"""
+    def operand(y):
+        m = _path(y) if paths else _member(y)
+        return m[1] if m is not None and m[0] == FIELD_DATA else None
+
+    if x.op == "cmp":
+        p = _json_leaf(x, paths)
+        if p is not None or (paths and x.a in ("in", "not in")):   # S in r[n1]..[nk] is membership, not a substring
+            return p
+    got = _str_leaf(x, operand)
+    if got is None:
+        return None
+    op, kind, name, consts = got
+    return kind, name, op, consts
 
 
 def field_index(fn):

@@ -1211,12 +1211,22 @@ def _match_text_fields(stage, inputs, programs=False):
                  dev.FIELD_VAL_ONE if vi is None else vi), op, mean, tuple(preds), expr
 
 
-def _match_json_fields(stage, inputs, programs=False):
+def _match_json_fields(stage, inputs, programs=False, paths=False):
     """map(json.loads) filter* keyed(r["k"] | int(r["k"]), 1 | r["v"] | int(r["v"]) | float(r["v"])) +
     PartialReduceCombiner(+ | min | max), or mean()'s keyed(key, (value, 1)) + component-wise (+, +), over text, each
     filter one lowering.json_predicate: (sources, (FIELD_SEP_JSON, key member, key kind, value member or FIELD_VAL_ONE),
     op, mean, device predicates, member names, (bare key, bare value)) or None. With `programs` each filter may be a
-    lowering.json_filter_program, as _match_text_fields takes filter programs."""
+    lowering.json_filter_program, as _match_text_fields takes filter programs. With `paths`, a stage that does not
+    match so may read member paths in its key, value and filters (lowering.json_fields_path_spec,
+    lowering.json_path_filter_program, which every filter of such a stage prefers): a member is then the tuple of its
+    names (a one-name path is its name), at most dev.JSON_MAX_NODES distinct path nodes. "m" in r[n1]..[nk] also lists
+    its container r[n1]..[nk], whose str the device tests for the substring."""
+    m = _match_json_stage(stage, inputs, programs, False)
+    return m if m is not None or not paths else _match_json_stage(stage, inputs, programs, True)
+
+
+def _match_json_stage(stage, inputs, programs, nested):
+    """_match_json_fields' match of stage: of the top-level members only, or (nested) of member paths"""
     if not isinstance(stage, GMap) or len(inputs) != 1:
         return None
     src = _text_files(inputs[0])
@@ -1230,12 +1240,16 @@ def _match_json_fields(stage, inputs, programs=False):
         return None
     keyed = ks[-1][1]
     spec = lowering.json_fields_spec(keyed.fn, keyed.fn2)
+    if spec is None and nested:
+        spec = lowering.json_fields_path_spec(keyed.fn, keyed.fn2)
     if spec is None:
         return None
     kname, kkind, vname, vkind, mean = spec
     members = []
 
     def member(name):
+        if isinstance(name, tuple) and len(name) == 1:
+            name = name[0]
         if name not in members:
             members.append(name)
         return members.index(name)
@@ -1244,8 +1258,10 @@ def _match_json_fields(stage, inputs, programs=False):
     vi = dev.FIELD_VAL_ONE if vname is None else member(vname)
     preds = []
     for _k, o in ks[1:-1]:
-        p = lowering.json_predicate(o.fn)
-        prog = [p] if p is not None else lowering.json_filter_program(o.fn) if programs else None
+        prog = lowering.json_path_filter_program(o.fn) if nested else None
+        if prog is None:
+            p = lowering.json_predicate(o.fn)
+            prog = [p] if p is not None else lowering.json_filter_program(o.fn) if programs else None
         if prog is None:
             return None
         for p in prog:
@@ -1255,7 +1271,13 @@ def _match_json_fields(stage, inputs, programs=False):
             kind, name, cmp, consts = p
             preds.append((dev.PRED_MEMBER if kind == lowering.FIELD_MEMBER else _PRED_KINDS[kind], member(name),
                           _PRED_CMPS.get(cmp, dev.CMP_EQ), consts))
-    if len(members) > dev.JSON_MAX_MEMBERS or not _preds_fit(preds):
+            if kind == lowering.FIELD_MEMBER and consts:   # the container, for the substring test of a str
+                member(name[:-1])
+    if nested and not any(isinstance(m, tuple) for m in members):
+        return None
+    if len(members) > dev.JSON_MAX_MEMBERS or not _preds_fit(preds) or \
+            len({m[:i] for m in members if isinstance(m, tuple) for i in range(1, len(m) + 1)} |
+                {(m,) for m in members if isinstance(m, str)}) > dev.JSON_MAX_NODES:
         return None
     binop = stage.options.get("binop")
     if mean:
@@ -1398,7 +1420,7 @@ def _lower_map(runner, stage, inputs, si):
             detail += " key=const" if len(expr[0][1]) == 1 and expr[0][1][0] & 0xFF == lowering.EV_CI else " key=expr"
         runner.stats.add(stage, "device text fields scan+combine", detail)
         return Frame(scan.keys, [scan.values], scalar=True, combined=True)
-    m = _match_json_fields(stage, inputs, programs=True)
+    m = _match_json_fields(stage, inputs, programs=True, paths=True)
     if m is not None:
         if dist.active():
             raise NotLowerable("the JSON field scan runs on one process")
@@ -1411,7 +1433,11 @@ def _lower_map(runner, stage, inputs, si):
                                                                       scan.host_lines)
         if preds:
             detail += " filtered=%d" % scan.filtered
-        runner.stats.add(stage, "device text fields scan+combine", detail + " sep=json")
+        detail += " sep=json"
+        nested = [p for p in members if isinstance(p, tuple)]
+        if nested:   # the longest member path, its names joined by '.'
+            detail += " path=" + ".".join(max(nested, key=len))
+        runner.stats.add(stage, "device text fields scan+combine", detail)
         return Frame(scan.keys, [scan.values], scalar=True, combined=True)
     if _match_line_count(stage, inputs):
         ds = inputs[0]

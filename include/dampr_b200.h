@@ -197,7 +197,8 @@ int32_t dampr_table_fallback_lines(dampr_ctx *ctx, dampr_table *t, uint64_t *lin
 #define DAMPR_PRED_INT 1      /* int(line.split(sep)[field]) against int64 constants                               */
 #define DAMPR_PRED_F64 2      /* float(line.split(sep)[field]) against one double (IEEE: NaN is unequal to all)    */
 #define DAMPR_PRED_NFIELDS 3  /* len(line.split(sep)) against one int64; `field` is unused                        */
-#define DAMPR_PRED_MEMBER 4   /* JSON scans only: "m" in r (DAMPR_CMP_IN) / "m" not in r (DAMPR_CMP_NOT_IN), n = 0  */
+#define DAMPR_PRED_MEMBER 4   /* JSON scans only: "m" in r (DAMPR_CMP_IN) / "m" not in r (DAMPR_CMP_NOT_IN), n = 0
+                                 (a call over member paths: n = 0 or 1, see the JSON block)                       */
 #define DAMPR_CMP_EQ 0
 #define DAMPR_CMP_NE 1
 #define DAMPR_CMP_LT 2
@@ -408,14 +409,33 @@ int32_t dampr_table_fetch_field_keys(dampr_ctx *ctx, dampr_table *t, dampr_textb
  *   or r["v"] is read bare learns from them that its column would hold another Python type.
  * - Predicates: STR takes a string member without escapes, INT a JSON integer of at most 18 digits, F64 any JSON
  *   number; a member of another type, or a missing one, makes the predicate undecided (a fallback line).
- *   DAMPR_PRED_MEMBER never is. */
+ *   DAMPR_PRED_MEMBER never is at the top level.
+ * - Paths: a member may be a path r[n1][n2]..[nk] of 2 .. DAMPR_JSON_MAX_PATH names, its bytes the names joined by
+ *   DAMPR_JSON_PATH_SEP (each name 1 .. DAMPR_JSON_MAX_NAME bytes). The names of all paths form at most
+ *   DAMPR_JSON_MAX_NODES distinct (parent, name) nodes, and no two members name the same path; an empty name in a
+ *   path, a longer path, more nodes or a repeated path return DAMPR_ERR_ARG. A call without a path runs exactly as
+ *   above. In a call with one:
+ *   - Every prefix r[n1]..[ni] (i < k) must be a present object for the member to be read. A missing or non-object
+ *     prefix (Python's KeyError / TypeError) makes a key or value read a fallback line, and any predicate on the
+ *     member undecided. "m" in r[n1]..[ni] is the member r[n1]..[ni][m] under DAMPR_PRED_MEMBER, decided when
+ *     r[n1]..[ni] is an object. Such a predicate may carry one STR constant (n = 1, the bytes of m): where
+ *     r[n1]..[ni] is itself a member of the call and a string without escapes, the predicate is the substring test
+ *     of m in it, as Python's `in` on a str. Under any other parent it is undecided.
+ *   - The last occurrence of a name wins at every level: a later duplicate of an interior name replaces its whole
+ *     subtree (`{"a":{"b":1},"a":{"c":2}}` has no r["a"]["b"]; `{"a":{"b":1},"a":5}` makes it a TypeError).
+ *   - Names are compared in the top-level object and in the objects of interior path names; a name with a backslash
+ *     in one of them makes the line a fallback line. Names elsewhere are skipped, escaped or not.
+ *   - The kinds, flags, number rules and limits above apply to a path's leaf as to a top-level member. */
 #define DAMPR_FIELD_SEP_JSON 257
 #define DAMPR_JSON_MAX_MEMBERS 8   /* members per call                                                                */
 #define DAMPR_JSON_MAX_NAME 64     /* bytes per member name: ASCII, no '"', '\\' or byte below 0x20                   */
 #define DAMPR_JSON_MAX_DEPTH 64    /* the top-level object is depth 1; a line nested deeper is a fallback line        */
+#define DAMPR_JSON_PATH_SEP 0x1F   /* joins the names of a path member                                               */
+#define DAMPR_JSON_MAX_PATH 4      /* names per path                                                                  */
+#define DAMPR_JSON_MAX_NODES 16    /* distinct (parent, name) nodes over a call's paths                              */
 typedef struct dampr_json_members {
     int32_t n;               /* 1 .. DAMPR_JSON_MAX_MEMBERS                                                       */
-    const char *bytes;       /* the names back to back                                                             */
+    const char *bytes;       /* the names (paths) back to back                                                     */
     const int32_t *len;      /* their lengths in bytes                                                             */
 } dampr_json_members;
 int32_t dampr_text_json_fields(dampr_ctx *ctx, dampr_table *t, dampr_textbuf *tb, uint64_t own_lo, uint64_t own_hi,

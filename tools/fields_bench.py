@@ -53,7 +53,9 @@ r[2] is the value, r[3] the quantity:
 "latency": float, "meta": {"user": "decoy", ...}, "pad": filler}, padded with JSON whitespace after the numbers, and
 runs `Dampr.json`-style stages: `map(json.loads).fold_by(r["user"], value=r["n"], +)` (--value float:
 float(r["latency"])), min / max / mean() the same way. The host-map rate is then json.loads plus the lambdas. The JSON
-line holds "format": "json"; --where is not taken.
+line holds "format": "json"; --where is not taken. --nested moves the key and the value one or two levels down:
+{"user": {"id": "u%07d"}, "stats": {"n": int, "status": .., "latency": float}, "meta": {"user": {"id": "decoy"}, ..},
+"pad": filler}, read as r["user"]["id"] and r["stats"]["n"] (float(r["stats"]["latency"])), and adds "nested": true.
 """
 import argparse
 import json
@@ -154,13 +156,19 @@ def whitespace_rows(text, seed, vwidth):
 JLINE = 176         # bytes per JSON line (--format json)
 
 
-def json_text(seed, n_lines, n_keys):
+JROW = '{"user":"u0000000","n":%s,"status":%s,"latency":%s,"meta":{"user":"decoy","ids":[%d,%d]},"pad":"'
+JROW_NESTED = '{"user":{"id":"u0000000"},"stats":{"n":%s,"status":%s,"latency":%s},' \
+    '"meta":{"user":{"id":"decoy"},"ids":[%d,%d]},"pad":"'
+
+
+def json_text(seed, n_lines, n_keys, nested=False):
     """n_lines seeded JSON lines of JLINE bytes: rows drawn from a pool of 4096 (int n, int-or-string status, float
-    latency, a nested decoy member named "user", a filler string), the user key u0000000..u{n_keys-1} (uniform)"""
+    latency, a nested decoy member named "user", a filler string), the user key u0000000..u{n_keys-1} (uniform);
+    nested: the rows of JROW_NESTED, the same members one level down"""
     prng = random.Random(seed)
     pool = np.empty((4096, JLINE), dtype=np.uint8)
     for i in range(len(pool)):
-        row = '{"user":"u0000000","n":%s,"status":%s,"latency":%s,"meta":{"user":"decoy","ids":[%d,%d]},"pad":"' % (
+        row = (JROW_NESTED if nested else JROW) % (
             str(prng.randrange(-99999, 100000)).ljust(7), str(prng.choice([200, 201, 404, 500, '"404"', '"503"'])).ljust(6),
             repr(prng.uniform(0, 1e3)).ljust(23), prng.randrange(1000), prng.randrange(1000))
         row += "".join(prng.choice("abcdefghij") for _ in range(JLINE - 3 - len(row))) + '"}\n'
@@ -268,10 +276,14 @@ def splitter(sep):
     return (lambda l: l.split()) if sep == "ws" else (lambda l: l.split(","))
 
 
-def json_job(Dampr, src, value, op):
+def json_job(Dampr, src, value, op, nested=False):
     d = Dampr.read_input(src).map(json.loads)
-    key = lambda r: r["user"]   # noqa: E731
-    val = (lambda r: r["n"]) if value == "int" else (lambda r: float(r["latency"]))
+    if nested:
+        key = lambda r: r["user"]["id"]   # noqa: E731
+        val = (lambda r: r["stats"]["n"]) if value == "int" else (lambda r: float(r["stats"]["latency"]))
+    else:
+        key = lambda r: r["user"]   # noqa: E731
+        val = (lambda r: r["n"]) if value == "int" else (lambda r: float(r["latency"]))
     if op == "mean":
         return d.mean(key, val)
     if op in ("min", "max"):
@@ -279,16 +291,18 @@ def json_job(Dampr, src, value, op):
     return d.fold_by(key, value=val, binop=lambda a, b: a + b)
 
 
-def json_rows(sample, value):
+def json_rows(sample, value, nested=False):
     """(key, value) of the sample's JSON lines, as the stage's lambdas read them"""
     for l in sample.decode("ascii").split("\n")[:-1]:
         r = json.loads(l)
+        if nested:
+            r = dict(r["stats"], user=r["user"]["id"])
         yield r["user"], (r["n"] if value == "int" else float(r["latency"]))
 
 
-def job(Dampr, src, value="int", op="sum", where="none", sep="comma", key_fields=1):
+def job(Dampr, src, value="int", op="sum", where="none", sep="comma", key_fields=1, nested=False):
     if sep == "json":
-        return json_job(Dampr, src, value, op)
+        return json_job(Dampr, src, value, op, nested)
     conv = int if value == "int" else float
     key = KEY_FNS[key_fields]
     d = Dampr.read_input(src)
@@ -304,7 +318,7 @@ def job(Dampr, src, value="int", op="sum", where="none", sep="comma", key_fields
     return d.fold_by(key, value=lambda r: conv(r[2]), binop=lambda a, b: a + b)
 
 
-def python_fold(sample, value, op, where="none", sep="comma", key_fields=1):
+def python_fold(sample, value, op, where="none", sep="comma", key_fields=1, nested=False):
     """the stage as plain Python over the sample's lines: {key: result}"""
     conv = int if value == "int" else float
     keep = WHERE.get(where, lambda r: True)
@@ -312,7 +326,7 @@ def python_fold(sample, value, op, where="none", sep="comma", key_fields=1):
     key = KEY_FNS[key_fields]
     out = {}
     if sep == "json":
-        rows = json_rows(sample, value)
+        rows = json_rows(sample, value, nested)
     else:
         lines = [l for l in sample.decode("ascii").split("\n")[:-1] if LINE_WHERE.get(where, lambda l: True)(l)]
         rows = ((key(r), conv(r[2])) for r in map(split, lines) if keep(r))
@@ -329,12 +343,12 @@ def python_fold(sample, value, op, where="none", sep="comma", key_fields=1):
     return out
 
 
-def magnitudes(sample, sep="comma", key_fields=1):
+def magnitudes(sample, sep="comma", key_fields=1, nested=False):
     """{key: (lines, sum of |float value|)} of the sample: the scale of the sum bound"""
     mag = {}
     split = splitter(sep)
     key = KEY_FNS[key_fields]
-    rows = json_rows(sample, "float") if sep == "json" else \
+    rows = json_rows(sample, "float", nested) if sep == "json" else \
         ((key(r), r[2]) for r in map(split, sample.decode("ascii").split("\n")[:-1]))
     for k, v in rows:
         n, a = mag.get(k, (0, 0.0))
@@ -378,6 +392,7 @@ def main():
                     default="none")
     ap.add_argument("--sep", choices=("comma", "ws", ","), default="comma")
     ap.add_argument("--format", choices=("csv", "json"), default="csv")
+    ap.add_argument("--nested", action="store_true", help="--format json: the key and value one or two levels down")
     ap.add_argument("--key-fields", type=int, choices=(1, 2, 3), default=1)
     ap.add_argument("--expr", choices=("none", "product", "ratio", "nfields"), default="none")
     ap.add_argument("--key", choices=("field", "const", "bucket"), default="field")
@@ -393,6 +408,8 @@ def main():
         if a.where != "none" or a.sep != "comma" or a.key_fields != 1:
             ap.error("--format json takes neither --where, --sep nor --key-fields")
         a.sep = "json"
+    elif a.nested:
+        ap.error("--nested takes --format json")
     if a.where == "int" and a.value != "int":
         ap.error("--where int needs --value int (int() of a float field raises)")
     default = a.value == "int" and a.op == "sum" and a.key_fields == 1 and not computed
@@ -405,7 +422,7 @@ def main():
     line = JLINE if a.sep == "json" else LINE
     n_lines = int(a.gb * 1e9) // line
     if a.sep == "json":
-        text = json_text(2026, n_lines, a.keys)
+        text = json_text(2026, n_lines, a.keys, a.nested)
     else:
         text = csv_text(2026, n_lines, a.keys) if a.value == "int" else float_text(2026, n_lines, a.keys)
         text = rewrite_filler(text, 2028, K)
@@ -436,7 +453,7 @@ def main():
         ctx.timings_reset()
         t0 = time.perf_counter()
         stage = expr_job(Dampr, src, a.expr, a.key, a.op, a.sep) if computed else \
-            job(Dampr, src, a.value, a.op, where, a.sep, K)
+            job(Dampr, src, a.value, a.op, where, a.sep, K, a.nested)
         n = len(list(stage.run()))
         dt = time.perf_counter() - t0
         stages = runner_mod.LAST_STATS.stages
@@ -476,12 +493,12 @@ def main():
             k, v = r[0], int(r[2])
             host[k] = host[k] + v if k in host else v
     else:
-        host = python_fold(sample, a.value, a.op, sep=a.sep, key_fields=K)
+        host = python_fold(sample, a.value, a.op, sep=a.sep, key_fields=K, nested=a.nested)
     host_s = time.perf_counter() - t0
     spin = dev.PinnedBuffer(len(sample))
     spin.array[:] = np.frombuffer(sample, dtype=np.uint8)
     got = dict((expr_job(Dampr, plan.MemoryText(spin.array), a.expr, a.key, a.op, a.sep) if computed else
-                job(Dampr, plan.MemoryText(spin.array), a.value, a.op, sep=a.sep, key_fields=K)).run())
+                job(Dampr, plan.MemoryText(spin.array), a.value, a.op, sep=a.sep, key_fields=K, nested=a.nested)).run())
 
     kernel_ms = min(m[1] for m in mem)
     res = {
@@ -506,7 +523,7 @@ def main():
         res.update({"value": a.value, "op": a.op,
                     "kernels_ms": {k: round(v, 3) for k, v in sorted(best[4].items())}})
         if a.value == "float" and a.op in ("sum", "mean"):
-            res["sample_within_bound"] = within_bound(got, host, magnitudes(sample, a.sep, K), a.op)
+            res["sample_within_bound"] = within_bound(got, host, magnitudes(sample, a.sep, K, a.nested), a.op)
         if computed:
             res.update({"expr": a.expr, "key": a.key})
             if a.expr == "ratio" or a.op == "mean":
@@ -535,6 +552,8 @@ def main():
         res["sep"] = "ws"
     if a.sep == "json":
         res["format"] = "json"
+    if a.nested:
+        res["nested"] = True
     if a.out is None:
         shutil.rmtree(tmpdir, ignore_errors=True)
     print(json.dumps(res))
